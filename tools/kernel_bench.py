@@ -4,9 +4,13 @@ Usage (on the GPU box): python tools/kernel_bench.py [--shape 75 2400 3600] [--d
 """
 
 import argparse
+import ctypes
+import hashlib
 import json
 import os
+import subprocess
 import sys
+import tempfile
 
 import torch
 
@@ -28,6 +32,23 @@ def time_call(fn, iters=10, warmup=3):
     return ts[len(ts) // 2], ts[0]
 
 
+def copy_stream_lib():
+    """tools/micro/copy_stream.cu (16-byte ld.global.cs / st.global.cs copy) built into a temporary directory,
+    keyed by the source hash, so the tree stays read-only."""
+    src = os.path.join(os.path.dirname(os.path.abspath(__file__)), "micro", "copy_stream.cu")
+    tag = hashlib.sha256(open(src, "rb").read()).hexdigest()[:16]
+    so = os.path.join(tempfile.gettempdir(), f"xgcm_b200_copy_stream_{tag}.so")
+    if not os.path.exists(so):
+        nvcc = os.path.join(os.environ.get("CUDA_HOME", "/usr/local/cuda"), "bin", "nvcc")
+        subprocess.run([nvcc, "-O3", "-shared", "-Xcompiler", "-fPIC", "-gencode", "arch=compute_90a,code=sm_90a",
+                        "-o", so + ".tmp", src], check=True)
+        os.replace(so + ".tmp", so)
+    lib = ctypes.CDLL(so)
+    lib.copy_stream.restype = ctypes.c_int
+    lib.copy_stream.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.c_int64, ctypes.c_int, ctypes.c_void_p]
+    return lib
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--shape", type=int, nargs="+", default=[75, 2400, 3600])
@@ -46,6 +67,13 @@ def main():
     y = torch.empty_like(x)
     med, best = time_call(lambda: y.copy_(x), args.iters)
     print(f"torch copy_            : {med:8.3f} ms  {2*cells*es/med/1e6:8.1f} GB/s (best {2*cells*es/best/1e6:.1f})")
+    lib = copy_stream_lib()
+    for bps in (4, 8):
+        y.zero_()
+        fn = lambda: lib.copy_stream(x.data_ptr(), y.data_ptr(), cells * es, bps, torch.cuda.current_stream().cuda_stream)
+        med, best = time_call(fn, args.iters)
+        assert torch.equal(x, y)
+        print(f"ld/st.global.cs copy {bps}x: {med:8.3f} ms  {2*cells*es/med/1e6:8.1f} GB/s (best {2*cells*es/best/1e6:.1f})")
     names = "ZYX" if len(args.shape) == 3 else [str(i) for i in range(len(args.shape))]
     for axis in range(len(args.shape)):
         for op in ("diff", "interp"):

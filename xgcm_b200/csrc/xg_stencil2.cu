@@ -7,10 +7,11 @@
 //
 // Any C-contiguous field collapses to (outer, n, inner) around the operated
 // axis.  Three kernels:
-//   k_stencil_strided  inner > 1 (Y, Z, ...): a warp owns 32 x VEC contiguous
-//       columns and marches J cells along the axis keeping the previous row in
-//       registers, so each input element is read once; U independent 16-byte
-//       loads are in flight per thread.
+//   k_stencil_plane  inner > 1 (Y, Z, ...): 8 lanes own one 128-byte line of a
+//       plane row and march J cells along the axis keeping the previous row in
+//       registers, so each input element is read once; a warp is 4 such strips,
+//       numbered flat over (plane, segment, line) (xg_plane.cuh); U independent
+//       16-byte loads are in flight per thread.
 //   k_stencil_row_vec  inner == 1 (X), aligned rows, n_out == n: a warp owns a
 //       512 B x U chunk of one row, the missing neighbour of each 16-byte
 //       vector comes from a warp shuffle, and only the chunk edge does one
@@ -22,6 +23,7 @@
 #include <stdlib.h>
 
 #include "xg_common.cuh"
+#include "xg_plane.cuh"
 #include "xg_stencil_tile.cuh"
 #include "xg_tma.cuh"
 
@@ -35,12 +37,10 @@ struct StencilArgs {
   int64_t nx_last;     // extent of the innermost dim (inner is a multiple of it when inner > 1)
   int lo, hi, bc;
   T fill;
-  int J;               // cells marched per warp-unit (strided kernel)
-  int64_t nseg, nwc;   // segments along the axis, warp-columns (or row chunks)
+  int64_t nwc;         // row chunks (row kernels)
   int64_t nunits;      // total warp-units
   bool small_units;    // nunits < 2^31: 32-bit unit decomposition
-  XgFastDiv fd_nseg, fd_nwc;  // multiply-high forms of nseg / nwc (valid with small_units)
-  bool seg_fast;       // unit order: segment index fastest (else warp-column fastest)
+  XgFastDiv fd_nwc;    // multiply-high form of nwc (valid with small_units)
   XgOperand pre, post;
   int pre_axis_vec_ok, post_axis_vec_ok;  // row kernels: metric vector loads along x
   const T* halo_lo;
@@ -53,28 +53,11 @@ constexpr int kWarpsPerBlock = kThreads / 32;
 // ---------------------------------------------------------------------------
 // strided-axis kernel
 // ---------------------------------------------------------------------------
-template <typename T, int VEC, int OP, bool MET, int U, int MINB = 4>
-__global__ void __launch_bounds__(kThreads, MINB)  // MINB = 4: <= 64 registers, 4 CTAs (1024 threads) per SM
-k_stencil_strided(const StencilArgs<T> a) {
+// output rows [j0, j1) of the VEC columns starting at inner index i of plane o
+template <typename T, int VEC, int OP, bool MET, int U>
+__device__ __forceinline__ void strided_march(const StencilArgs<T>& a, int64_t o, int64_t i, int64_t j0,
+                                              int64_t j1) {
   typedef XgPack<T, VEC> Pack;
-  const int64_t unit =
-      (int64_t)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
-  if (unit >= a.nunits) return;
-  const int lane = threadIdx.x & 31;
-  int64_t wc, t, seg, o;
-  if (a.seg_fast) {  // segments of one column group adjacent in launch order
-    xg_divmod(unit, a.nseg, a.fd_nseg, a.small_units, t, seg);
-    xg_divmod(t, a.nwc, a.fd_nwc, a.small_units, o, wc);
-  } else {
-    xg_divmod(unit, a.nwc, a.fd_nwc, a.small_units, t, wc);
-    xg_divmod(t, a.nseg, a.fd_nseg, a.small_units, o, seg);
-  }
-  const int64_t i = (wc * 32 + lane) * VEC;
-  if (i >= a.inner) return;
-
-  const int64_t j0 = seg * a.J;
-  const int64_t j1 = (j0 + a.J < a.n_out) ? (j0 + a.J) : a.n_out;
-
   const T* ibase = a.in + o * a.n * a.inner + i;
   T* obase = a.out + o * a.n_out * a.inner + i;
   const bool has_pre = MET && a.pre.ptr != nullptr;
@@ -168,6 +151,26 @@ k_stencil_strided(const StencilArgs<T> a) {
     emit(j, prev, cur);
     prev = cur;
   }
+}
+
+// ---------------------------------------------------------------------------
+// plane-strided kernel (xg_plane.cuh): a warp = LPW strips of one 128-byte line x J rows, numbered flat
+// over (plane, segment, line)
+// ---------------------------------------------------------------------------
+template <typename T, int VEC>
+struct PlaneGeo {
+  static constexpr int LPL = 128 / (VEC * (int)sizeof(T));  // lanes per 128-byte line
+  static constexpr int LPW = 32 / LPL;                      // lines per warp
+};
+
+template <typename T, int VEC, int OP, bool MET, int U>
+__global__ void __launch_bounds__(kThreads, 4)  // <= 64 registers, 4 CTAs (1024 threads) per SM
+k_stencil_plane(const StencilArgs<T> a, const XgPlanePlan p) {
+  constexpr int LPL = PlaneGeo<T, VEC>::LPL, LPW = PlaneGeo<T, VEC>::LPW;
+  const int64_t w = (int64_t)blockIdx.x * kWarpsPerBlock + (threadIdx.x >> 5);
+  if (w >= p.nwarps) return;
+  xg_plane_walk(p, a.inner, a.n_out, LPL, LPW, VEC, w, threadIdx.x & 31,
+                [&](int64_t o, int64_t i, int64_t j0, int64_t j1) { strided_march<T, VEC, OP, MET, U>(a, o, i, j0, j1); });
 }
 
 // ---------------------------------------------------------------------------
@@ -710,43 +713,22 @@ static int env_int(const char* name, int dflt) {
 }
 
 template <typename T, int VEC, int OP, bool MET>
-int launch_strided(StencilArgs<T>& a, cudaStream_t st) {
-  const int64_t nvec = xg_ceil_div(a.inner, VEC);
-  a.nwc = xg_ceil_div(nvec, 32);
-  // march length: long enough that the re-read halo row is a few % of traffic,
-  // short enough that there are plenty of warps for every SM.
-  static const int tune_j = env_int("XG_STRIDED_J", 0);  // tuning knobs (benchmarks only)
-  static const int tune_u = env_int("XG_STRIDED_U", 0);
-  // Tuning notes (not repeated on H100): in a loop of identical launches short marches (J = 4)
-  // look faster for Y, but the mixed sequence of bench.py shows no gain, and the fused-metric
-  // variants lose (per-segment operand setup is amortised over fewer rows) — so 32 stays; a
-  // plane-strided axis marches as far as possible.
-  int J;
-  if (tune_j > 0) J = tune_j;
-  else J = (a.n_out <= 96) ? (int)a.n_out : 32;
-  if (J > a.n_out) J = (int)a.n_out;
-  a.J = J;
-  a.nseg = xg_ceil_div(a.n_out, J);
-  a.nunits = a.outer * a.nseg * a.nwc;
-  a.small_units = a.nunits < (1ll << 31);
-  a.fd_nseg = xg_fastdiv_make(a.small_units ? a.nseg : 1);
-  a.fd_nwc = xg_fastdiv_make(a.small_units ? a.nwc : 1);
-  static const int tune_sf = env_int("XG_STRIDED_SEGFAST", 0);
-  a.seg_fast = tune_sf != 0;
-  const int64_t blocks = xg_ceil_div(a.nunits, kWarpsPerBlock);
+int launch_plane(StencilArgs<T>& a, cudaStream_t st) {
+  typedef PlaneGeo<T, VEC> G;
+  constexpr int U = 4;
+  auto kern = k_stencil_plane<T, VEC, OP, MET, U>;
+  // Rows per strip: the whole axis when it is short (Z of a (Z, Y, X) field: no segment boundaries at all), else
+  // J = 4.  Short strips keep the warps resident at one time on a compact, contiguous part of a plane (strips are
+  // numbered plane, segment, line), and a segment's first row, the previous segment's last, is re-read from L2
+  // while that segment is still running.  On H100 (Y of the C3 field) J = 4 beat 8, 16 and 32, which lost 4 % and
+  // more; long marches by persistent warps lost more still.  The metric-fused forms keep J = 32: their operand
+  // setup is paid per strip.
+  const int64_t J = (a.n_out <= 96) ? a.n_out : (MET ? 32 : 4);
+  const XgPlanePlan p = xg_plane_plan(a.outer, a.inner, a.n_out, G::LPL * VEC, G::LPW, J);
+  const int64_t blocks = xg_ceil_div(p.nwarps, kWarpsPerBlock);
   if (blocks > 0x7fffffffLL) return xg_fail(XG_EINVAL, "xg_stencil2: grid too large");
-  static const int tune_met = env_int("XG_STRIDED_MET", 0);  // 1: U=2; 2: U=4 at 3 CTAs/SM (80 registers)
-  if (!MET && tune_u == 8)
-    k_stencil_strided<T, VEC, OP, MET, 8><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  else if (!MET && tune_u == 2)
-    k_stencil_strided<T, VEC, OP, MET, 2><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  else if (MET && VEC > 1 && tune_met == 1)
-    k_stencil_strided<T, VEC, OP, MET, 2><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  else if (MET && VEC > 1 && tune_met == 2)
-    k_stencil_strided<T, VEC, OP, MET, 4, 3><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  else
-    k_stencil_strided<T, VEC, OP, MET, 4><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  return xg_check_launch("xg_stencil2(strided)");
+  kern<<<(unsigned)blocks, kThreads, 0, st>>>(a, p);
+  return xg_check_launch("xg_stencil2(plane)");
 }
 
 template <typename T, int VEC, int OP, bool MET>
@@ -1029,10 +1011,10 @@ int dispatch_layout(StencilArgs<T>& a, cudaStream_t st) {
         }
       }
     }
-    if (ptr_ok && a.inner % VEC == 0) return launch_strided<T, VEC, OP, MET>(a, st);
+    if (ptr_ok && a.inner % VEC == 0) return launch_plane<T, VEC, OP, MET>(a, st);
     a.pre.vec_ok = 0;
     a.post.vec_ok = 0;
-    return launch_strided<T, 1, OP, MET>(a, st);
+    return launch_plane<T, 1, OP, MET>(a, st);
   }
   if (ptr_ok && a.n_out == a.n && a.n % VEC == 0 && a.n / VEC >= 32) {
     if constexpr (MET) {
@@ -1097,10 +1079,8 @@ int stencil2_typed(int op, const void* in, void* out, int ndim, const int64_t* s
   a.fill = static_cast<T>(fill_value);
   a.halo_lo = static_cast<const T*>(halo_lo);
   a.halo_hi = static_cast<const T*>(halo_hi);
-  a.J = 0;
-  a.nseg = a.nwc = a.nunits = 0;
+  a.nwc = a.nunits = 0;
   a.small_units = false;
-  a.seg_fast = false;
   if (v.n == 0) return xg_fail(XG_EINVAL, "xg_stencil2: empty operated axis");
   if (v.outer == 0 || v.inner == 0 || a.n_out <= 0) return XG_OK;  // nothing to write
 

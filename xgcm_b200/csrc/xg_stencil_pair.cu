@@ -12,7 +12,7 @@
 //     ta = OPa(A x ma), tb = OPb(B x mb), s = ta +- tb, out = s / post   — each rounded to the field dtype.
 // Both stencils are length preserving (lo + hi == 1: center <-> left / right), so A, B and out share one shape.
 //
-// Work split (as k_stencil_strided): a warp owns 32 x VEC contiguous cells of the innermost dim and marches J
+// Work split: a warp owns 32 x VEC contiguous cells of the innermost dim and marches J
 // cells along axis b keeping B's previous row in registers; the x-neighbour of A comes from a warp shuffle,
 // only the lanes at a warp or row edge do one extra scalar load (or take the boundary value).
 #include <stdlib.h>

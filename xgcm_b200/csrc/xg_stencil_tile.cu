@@ -5,7 +5,7 @@
 //     out = ( OPa(pad_a(A x ma)) along x   (+|-)   OPb(pad_b(B x mb)) along p ) / post        (z, p, x) view
 //
 // Replaces, per call, the chain xgcm/grid.py:796-832 (+ one xarray arithmetic pass per operator) exactly
-// like k_stencil_strided / k_stencil_pair do; what changes is the data movement:
+// like k_stencil_plane / k_stencil_pair do; what changes is the data movement:
 //   * a tile is U = 4 levels x TY output rows x TXE cells; every operand of the tile is ONE bulk tensor
 //     load (cp.async.bulk.tensor, SASS UTMALDG): A with a 16-byte halo along x, B with one halo row
 //     along p, the metrics as 2-D boxes (shared between levels: loaded once per tile, not per level) or as
