@@ -18,6 +18,7 @@
  *   xg_pad             <- xgcm/padding.py:765-871 (pad) for callers that want the
  *                         padded array itself (custom grid ufuncs)
  *   xg_strided_copy    <- xgcm/padding.py:260-572 (_pad_face_connections: one connected edge)
+ *   xg_fold_rows       <- xgcm/padding.py:619-684 (_fold_north_halo: the north-fold halo rows)
  *   xg_binary / xg_unary
  *                      <- the xarray broadcast arithmetic around the hot path
  *                         (xgcm/grid.py:808,832,1578,1599,1657)
@@ -226,6 +227,25 @@ XG_API int xg_binary(int binop, int dtype, const void* a, const void* b,
 XG_API int xg_strided_copy(int dtype, void* dst, const int64_t* dst_strides, const void* src,
                     const int64_t* src_strides, int ndim, const int64_t* shape, int negate,
                     void* stream);
+
+/*
+ * North-fold halo of a tripolar grid (xgcm/padding.py:619-684): `width` rows of the field `in`
+ * (`shape`, contiguous) mirrored across the fold, written into `out`, which has `in`'s shape except
+ * `out_len` along fold_axis:
+ *
+ *   out[..., row0 + r, ..., k, ...] = (negate ? -1 : 1) * (in * pre)[..., n-1-skip-r, ..., (mirror - k) mod period, ...]
+ *
+ * for r < width along fold_axis and every k along seam_axis (either order; other dims are copied
+ * through).  `pre` (optional) broadcasts against `in` via pre_strides and is read at the mirrored
+ * cell, like the halo planes xg_stencil2 takes as already metric-weighted.  The plane of xg_stencil2
+ * is out_len = 1, row0 = 0, width = 1; the north rows of a padded array are out_len = n + width,
+ * row0 = n.  XG_EINVAL for null pointers, fold_axis == seam_axis, width < 1 or width > n - skip;
+ * XG_ENOTIMPL if a mirror partner lies outside the seam dim (an `inner` seam under a center pivot).
+ */
+XG_API int xg_fold_rows(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                        int fold_axis, int seam_axis, int64_t out_len, int64_t row0, int width,
+                        int skip, int64_t mirror, int64_t period, int negate, const void* pre,
+                        const int64_t* pre_strides, void* stream);
 
 /*
  * `count` strided copies of the same rank in ONE launch (all connected edges of a field:

@@ -75,6 +75,11 @@ SIGNATURES = {
         [C.c_int, C.c_int, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_int, _i64p, _i64p, _i64p,
          C.POINTER(C.c_int), _vp],
     ),
+    "xg_fold_rows": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int,
+         C.c_int64, C.c_int64, C.c_int, _vp, _i64p, _vp],
+    ),
     "xg_binary": (C.c_int, [C.c_int, C.c_int, _vp, _vp, _i64p, _vp, C.c_int, _i64p, _vp]),
     "xg_fill_uniform": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_uint64, C.c_uint64, _vp]),
     "xg_fill_uniform_host": (C.c_int, [C.c_int, _vp, C.c_int64, C.c_uint64, C.c_uint64]),

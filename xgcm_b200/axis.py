@@ -12,6 +12,7 @@ from __future__ import annotations
 from typing import Mapping, Optional, Tuple, Union
 
 from .labeled import Dataset
+from .padding import _parse_fold_padding
 
 VALID_POSITION_NAMES = "center|left|right|inner|outer"
 _VALID_POSITIONS = tuple(VALID_POSITION_NAMES.split("|"))
@@ -94,11 +95,9 @@ class Axis:
                 raise ValueError(f"Can't set the default shift for {pos} to be to {pos}")
 
         if isinstance(padding, Mapping):
-            raise NotImplementedError(
-                "north-fold padding specs are outside the scope of xgcm_b200 "
-                "(experimental topology feature of the reference, padding.py:21-181)"
-            )
-        if padding is not None and padding not in VALID_PADDINGS + EXTENSION_PADDINGS:
+            # a north-fold spec, e.g. {"fold": "corner"}; its seam axis is inferred by Grid._validate_folds
+            padding = _parse_fold_padding(padding)
+        elif padding is not None and padding not in VALID_PADDINGS + EXTENSION_PADDINGS:
             raise ValueError(
                 f"padding must be one of {list(VALID_PADDINGS)} "
                 f"or a fold spec (e.g. {{'fold': 'corner'}}) or None, but got {padding}"
@@ -136,7 +135,7 @@ class Axis:
         return self._default_shifts
 
     @property
-    def padding(self) -> Optional[str]:
+    def padding(self) -> Optional[Union[str, Mapping]]:
         return self._padding
 
     @property

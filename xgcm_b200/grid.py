@@ -15,8 +15,13 @@ produced by a CUDA kernel behind the C-ABI:
 * ``transform`` (linear / log): ``xg_vinterp_linear`` (transform.py).
 
 Host (numpy-backed) inputs are streamed through the GPU and come back as numpy;
-CUDA-resident inputs stay resident.  Out of scope (raise ``NotImplementedError``):
-north-fold padding, dask chunking.
+CUDA-resident inputs stay resident.
+
+A north fold (tripolar grids, ``padding={"X": "periodic", "Y": {"fold": pivot}}``,
+reference grid.py:411-470) is recorded in ``grid._folds``; an operator across it
+takes the folded row as a halo plane of its ``xg_stencil2`` launch (one
+``xg_fold_rows`` launch beside it).  Out of scope (raise ``NotImplementedError``):
+dask chunking.
 """
 
 from __future__ import annotations
@@ -41,7 +46,7 @@ from .grid_ufunc import (
 )
 from .labeled import DataArray, Dataset, is_device_array
 from .metrics import iterate_axis_combinations
-from .padding import pad  # noqa: F401  (re-exported like the reference's grid module)
+from .padding import fold_edges, pad  # noqa: F401  (pad: re-exported like the reference's grid module)
 
 
 def _maybe_promote_str_to_list(a):
@@ -117,7 +122,6 @@ class Grid:
         else:
             self._facedim = None
             self._face_connections = None
-        self._folds = {}
 
         all_axes = list(coords.keys())
         padding_dict = self._map_kwargs_over_axes(padding, axes=all_axes)
@@ -138,6 +142,7 @@ class Grid:
 
         if face_connections is not None:
             self._assign_face_connections(face_connections)
+        self._validate_folds()
 
         self._metrics: Dict[frozenset, List[DataArray]] = {}
         self._metric_cache: Dict[Any, Any] = {}
@@ -205,6 +210,40 @@ class Grid:
         for axis, axis_links in axis_connections.items():
             self.axes[axis]._facedim = facedim
             self.axes[axis]._face_connections = axis_links
+
+    def _validate_folds(self):
+        """Record every north fold in ``self._folds[fold axis] = {"seam_axis", "pivot", "south"}``
+        (grid.py:411-470).  The seam is the one OTHER axis whose padding was given as "periodic";
+        an axis with no padding is not a candidate."""
+        self._folds: Dict[str, Dict[str, Any]] = {}
+        for axname, axis in self.axes.items():
+            spec = axis._padding
+            if not isinstance(spec, Mapping):
+                continue
+            seams = [other for other in self.axes if other != axname and other in self._explicitly_periodic_axes]
+            if not seams:
+                raise ValueError(
+                    f"A fold padding on axis {axname!r} requires an explicitly periodic seam axis (the zonal "
+                    "wrap), but no other axis was explicitly marked periodic. Set e.g. "
+                    "padding={'X': 'periodic', '" + str(axname) + "': {'fold': ...}}."
+                )
+            if len(seams) > 1:
+                raise ValueError(
+                    f"A fold padding on axis {axname!r} is ambiguous: more than one explicitly periodic "
+                    f"axis could be the seam ({seams}). Multiple candidate seam axes are not supported."
+                )
+            self._folds[axname] = {"seam_axis": seams[0], "pivot": spec["fold"], "south": spec["south"]}
+        if self._folds and self._face_connections is not None:
+            raise NotImplementedError(
+                "Combining a north-fold boundary with face_connections is not supported "
+                f"(fold axes: {sorted(self._folds)}). Use one or the other."
+            )
+        if self._folds:
+            warnings.warn(
+                "The north-fold (tripolar) boundary condition is experimental. Its API and numerical "
+                "behavior may change in future releases; please review results carefully.",
+                category=UserWarning,
+            )
 
     # ------------------------------------------------------------------ kwargs plumbing
     def _map_kwargs_over_axes(self, kwargs, axes: Optional[Iterable[str]] = None) -> Dict[str, Any]:
@@ -548,7 +587,9 @@ class Grid:
                 out_dim = self.axes[ax_name].coords[to_pos]
             except KeyError:
                 raise ValueError(f"Axis position ({ax_name}:{to_pos}) does not exist in grid")
-            pad_mode = paddings[ax_name]
+            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
+            if folded:
+                return None  # the fold row is a halo plane of the per-axis launch
             if (lo or hi) and pad_mode is None:
                 raise ValueError(
                     f"No boundary condition was specified for axis {ax_name!r}, but the "
@@ -619,7 +660,9 @@ class Grid:
                 out_dim = self.axes[ax_name].coords[to_pos]
             except KeyError:
                 raise ValueError(f"Axis position ({ax_name}:{to_pos}) does not exist in grid")
-            pad_mode = paddings[ax_name]
+            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
+            if folded:
+                return one_by_one()  # the host pipeline takes no halo planes
             if (lo or hi) and pad_mode is None:
                 raise ValueError(
                     f"No boundary condition was specified for axis {ax_name!r}, but the "
@@ -648,7 +691,7 @@ class Grid:
 
     # ------------------------------------------------------------------ two-field composites (extension)
     def pair(self, funcname_a, da_a, axis_a, funcname_b, da_b, axis_b, combine="add", metric_a=None,
-             metric_b=None, divide_by=None, to=None, padding=None, fill_value=None):
+             metric_b=None, divide_by=None, to=None, padding=None, fill_value=None, _components=None):
         """``(f_a(da_a * metric_a, axis_a)  +|-  f_b(da_b * metric_b, axis_b)) / metric_out`` — what users chain
         from ``Grid.diff`` / ``Grid.interp`` and xarray arithmetic for divergence-like quantities
         (docs/ufunc_examples.md:105-153), evaluated in ONE kernel (``xg_stencil_pair``) when both terms are
@@ -656,7 +699,10 @@ class Grid:
 
         ``metric_a`` / ``metric_b``: axes whose metric (``get_metric`` at the input's position) multiplies the
         input; ``divide_by``: axes whose metric at the OUTPUT position divides the result; ``combine``: "add" or
-        "sub" (term a minus term b).  Anything the fused kernel does not cover runs as the explicit chain."""
+        "sub" (term a minus term b).  Anything the fused kernel does not cover runs as the explicit chain.
+
+        ``_components``: the vector-component axes of ``da_a`` / ``da_b`` (divergence, vorticity); a term
+        across a north fold then folds its input as that component, which changes its sign."""
         from . import ops
         from .device import as_device_tensor, result_like
 
@@ -680,6 +726,9 @@ class Grid:
         def chain():
             xa = da_a * self.get_metric(da_a, metric_a) if metric_a else da_a
             xb = da_b * self.get_metric(da_b, metric_b) if metric_b else da_b
+            if _components is not None:
+                xa = {_components[0]: xa} if axis_a in self._folds else xa
+                xb = {_components[1]: xb} if axis_b in self._folds else xb
             ta = self._1d_grid_ufunc_dispatch(funcname_a, xa, axis_a, to={axis_a: to.get(axis_a)}, **kw)
             tb = self._1d_grid_ufunc_dispatch(funcname_b, xb, axis_b, to={axis_b: to.get(axis_b)}, **kw)
             if ta.dims != tb.dims:
@@ -706,10 +755,11 @@ class Grid:
             from_pos, to_pos = sig.in_ax_positions[0][0], sig.out_ax_positions[0][0]
             in_dim = self.axes[ax_name].coords[from_pos]
             out_dim = self.axes[ax_name].coords.get(to_pos)
-            if out_dim is None or lo + hi != 1 or paddings[ax_name] not in ("periodic", "fill", "extend"):
+            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
+            if folded or out_dim is None or lo + hi != 1 or pad_mode not in ("periodic", "fill", "extend"):
                 return chain()
             fv = fills[ax_name] if fills[ax_name] is not None else 0.0
-            terms.append(dict(op=funcname, lo=lo, hi=hi, pad=paddings[ax_name], fill=fv, axn=da.get_axis_num(in_dim),
+            terms.append(dict(op=funcname, lo=lo, hi=hi, pad=pad_mode, fill=fv, axn=da.get_axis_num(in_dim),
                               in_dim=in_dim, out_dim=out_dim, ax=ax_name))
         ta, tb = terms
         out_dims_a = tuple(ta["out_dim"] if d == ta["in_dim"] else d for d in da_a.dims)
@@ -750,12 +800,12 @@ class Grid:
         """Finite-volume horizontal divergence ``(diff(u * dy, X) + diff(v * dx, Y)) / area`` on a C-grid, metrics
         from ``get_metric`` (u * its Y-metric, v * its X-metric, area at the output position); one fused pass."""
         return self.pair("diff", u, axis_u, "diff", v, axis_v, combine="add", metric_a=(axis_v,), metric_b=(axis_u,),
-                         divide_by=(axis_u, axis_v), **kwargs)
+                         divide_by=(axis_u, axis_v), _components=(axis_u, axis_v), **kwargs)
 
     def vorticity(self, u, v, axis_u="X", axis_v="Y", **kwargs):
         """Vertical relative vorticity ``(diff(v * dy, X) - diff(u * dx, Y)) / area`` on a C-grid; one fused pass."""
         return self.pair("diff", v, axis_u, "diff", u, axis_v, combine="sub", metric_a=(axis_v,), metric_b=(axis_u,),
-                         divide_by=(axis_u, axis_v), **kwargs)
+                         divide_by=(axis_u, axis_v), _components=(axis_v, axis_u), **kwargs)
 
     def apply_as_grid_ufunc(self, func: Callable, *args, axis=None, signature="", padding_width=None,
                             padding=None, fill_value=None, dask="forbidden", map_overlap=False,
@@ -843,7 +893,8 @@ class Grid:
         # numpy-backed field, one axis: stream slabs through the GPU (xg_cumscan_host) instead of one
         # un-overlapped upload + download around the kernel
         host_stream = (host_input and len(axis) == 1 and self._face_connections is None
-                       and np.asarray(da.data).dtype in (np.float32, np.float64))
+                       and np.asarray(da.data).dtype in (np.float32, np.float64)
+                       and axis[0] not in self._folds)  # (the slab pipeline takes no fold halo)
         if host_stream:
             data = da
         else:
@@ -865,7 +916,7 @@ class Grid:
                     f"From `{pos}` to `{ax_to}` is not a valid position "
                     f"shift for cumsum operation along axis {ax}."
                 )
-            ax_padding = paddings[ax.name]
+            folded, ax_padding = fold_edges(self, ax.name, paddings[ax.name], pad_hi)
             if (pad_lo or pad_hi) and ax_padding is None and self._face_connections is None:
                 raise ValueError(
                     f"No boundary condition was specified for axis {ax.name!r}, but the "
@@ -900,10 +951,11 @@ class Grid:
                     else:  # two roundings in the reference, (da * w) * metric: keep them
                         data = data._replace(data=ops.binary("mul", data.data, w_t))
             fv = fills[ax.name] if fills[ax.name] is not None else 0.0
-            if self._face_connections is not None and (pad_lo or pad_hi):
+            if (self._face_connections is not None and (pad_lo or pad_hi)) or folded:
                 # the reference pads the cumsum'd data with ``pad`` (grid.py:1385-1391), which on a
-                # connected grid takes the halo from the neighbour face: scan + trim in the
-                # kernel, halo through the face-connection padding, metric divide last
+                # connected grid takes the halo from the neighbour face and across a north fold
+                # mirrors the scanned rows: scan + trim in the kernel, halo through ``pad``, metric
+                # divide last
                 y = ops.cumscan(data.data, axis_num, ax_reverse, trim, 0, 0, None, fv, pre=pre_t,
                                 post=None, skipna=True)
                 scanned = DataArray(y, dims=data.dims, name=da.name, attrs=da.attrs)

@@ -599,10 +599,12 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             op, da, da if raw_arg is None else raw_arg, other_component, grid, ax_name, in_dim,
             out_dim, padding_width_real, padding, fill_value, pre_metric, post_metric_fn,
         )
+    from .padding import fold_edges, fold_halo_plane
+
     lo, hi = padding_width_real.get(ax_name, (0, 0))
     paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
     fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
-    ax_padding = paddings[ax_name]
+    folded, ax_padding = fold_edges(grid, ax_name, paddings[ax_name], hi)
     if (lo or hi) and ax_padding is None:
         raise ValueError(
             f"No boundary condition was specified for axis {ax_name!r}, but the "
@@ -611,8 +613,6 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
             f"grid method."
         )
-    if isinstance(ax_padding, (dict, collections.abc.Mapping)):
-        raise NotImplementedError("fold padding is outside the scope of xgcm_b200")
     axis_num = da.get_axis_num(in_dim)
     out_dims = tuple(out_dim if d == in_dim else d for d in da.dims)
     out_shape = list(da.shape)
@@ -621,7 +621,8 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
     bc = ax_padding if (lo or hi) else None
     fv = fills[ax_name] if fills[ax_name] is not None else 0.0
 
-    if not da.is_device and isinstance(da.data, np.ndarray) and da.data.dtype in (np.float32, np.float64):
+    if (not folded and not da.is_device and isinstance(da.data, np.ndarray)
+            and da.data.dtype in (np.float32, np.float64)):
         # host field: stream slabs H2D -> kernel -> D2H inside the library (xg_stencil2_host)
         try:
             out = ops.stencil2_host(
@@ -637,7 +638,14 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
     x, was_host = as_device_tensor(da.data, grid._device_for(da))
     pre_t = grid._metric_tensor(pre_metric, da.dims, x) if pre_metric is not None else None
     post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
-    out = ops.stencil2(x, axis_num, op, lo, hi, bc, fv, pre=pre_t, post=post_t)
+    halo_lo = halo_hi = None
+    if folded:
+        # the north halo is the folded row (of x * pre, sign-flipped for a vector component); a periodic
+        # south edge wraps the row above the top, which is that same fold row (reference padding.py:723-762)
+        halo_hi = fold_halo_plane(grid, ax_name, da.dims, x, pre=pre_t, negate=isinstance(raw_arg, dict))
+        if lo and ax_padding == "periodic":
+            halo_lo = halo_hi
+    out = ops.stencil2(x, axis_num, op, lo, hi, bc, fv, pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
     return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
 
 

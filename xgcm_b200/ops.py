@@ -204,6 +204,39 @@ def pad(x: torch.Tensor, axis: int, lo: int, hi: int, padding: Optional[str],
     return out
 
 
+def fold_rows(x: torch.Tensor, fold_axis: int, seam_axis: int, width: int, skip: int, mirror: int,
+              period: int, negate: bool = False, pre: Optional[torch.Tensor] = None,
+              out: Optional[torch.Tensor] = None, row0: int = 0) -> torch.Tensor:
+    """North-fold halo rows (xg_fold_rows): ``out[..., row0 + r, ..., k, ...] = +-(x * pre)[..., n-1-skip-r, ...,
+    (mirror - k) mod period, ...]`` for ``r < width`` along ``fold_axis`` and every ``k`` along ``seam_axis``.
+
+    Without ``out`` the result holds just the ``width`` rows (``width = 1``: the halo plane of
+    :func:`stencil2`); with ``out`` (contiguous, ``x``'s shape but any length along ``fold_axis``) the rows
+    land at ``row0`` of it."""
+    lib = _capi.load()
+    _require_cuda(x, "field")
+    x = x.contiguous()
+    fold_axis = _norm_axis(fold_axis, x.dim())
+    seam_axis = _norm_axis(seam_axis, x.dim())
+    shape = list(x.shape)
+    if out is None:
+        out_shape = list(shape)
+        out_shape[fold_axis] = int(width)
+        out = torch.empty(out_shape, dtype=x.dtype, device=x.device)
+    else:
+        _require_cuda(out, "out")
+        same = [s for d, s in enumerate(out.shape) if d != fold_axis] == [s for d, s in enumerate(shape) if d != fold_axis]
+        if out.dim() != x.dim() or not same or out.dtype != x.dtype or not out.is_contiguous():
+            raise ValueError("out has wrong shape/dtype/layout")
+    keep_pre, pre_ptr, pre_st = _operand(pre, shape, x, "pre metric")
+    with torch.cuda.device(x.device):
+        rc = lib.xg_fold_rows(_dtype_code(x), x.data_ptr(), out.data_ptr(), x.dim(), _capi.i64_array(shape),
+                              fold_axis, seam_axis, int(out.shape[fold_axis]), int(row0), int(width), int(skip),
+                              int(mirror), int(period), 1 if negate else 0, pre_ptr, pre_st, _stream_ptr(x))
+    _capi.check(rc)
+    return out
+
+
 def strided_copy(dst: torch.Tensor, dst_offset: int, dst_strides: Sequence[int],
                  src: torch.Tensor, src_offset: int, src_strides: Sequence[int],
                  shape: Sequence[int], negate: bool = False) -> None:

@@ -10,8 +10,14 @@ are pre-padded with the ordinary boundary condition, then the halo of every
 connected edge is overwritten with the neighbour face's rim — sliced, swapped,
 flipped and sign-flipped as the connection demands.  Each of those edge
 transfers is one ``xg_strided_copy`` launch whose signed strides encode the
-whole index map.  North-fold padding (padding.py:21-181, :619-762) is out of
-scope.
+whole index map.
+
+On grids with a north fold (tripolar ocean grids, ``padding={"X": "periodic",
+"Y": {"fold": pivot}}``, reference padding.py:21-181, :619-762) the north edge of
+the fold axis is padded by ``_pad_fold``: its halo rows are interior rows mirrored
+along the periodic seam axis about the pole (``xg_fold_rows``), the south edge
+and every other axis are padded as usual, in that order.  Operators take the
+folded row as a halo plane of the fused stencil (``fold_halo_plane``).
 """
 
 from __future__ import annotations
@@ -26,6 +32,185 @@ _XGCM_BOUNDARY_KWARG_TO_XARRAY_PAD_KWARG = {
     "fill": "constant",
     "extend": "edge",
 }
+
+# ---------------------------------------------------------------------------------------------- north fold
+# The pivot names the sublattice the pole sits on along the seam (X) and fold (Y) axes: a cell
+# centre or a cell edge (T / F / U / V points of ocean models).  The fold is experimental in the
+# reference too; Grid construction warns.
+_PIVOT_ALIASES = {
+    "center": {"seam": "center", "fold": "center"},
+    "t": {"seam": "center", "fold": "center"},
+    "corner": {"seam": "edge", "fold": "edge"},
+    "f": {"seam": "edge", "fold": "edge"},
+    "u": {"seam": "edge", "fold": "center"},
+    "v": {"seam": "center", "fold": "edge"},
+}
+
+# seam position -> (2 * offset of its cell coordinate, cells - length); the mirror partner of seam
+# index k is (C - k - 2 * offset) mod N with N the number of cells, C = 0 (edge pivot) or 1 (centre)
+_SEAM_POSITION = {"center": (1, 0), "left": (0, 0), "right": (2, 0), "outer": (0, -1), "inner": (2, 1)}
+
+
+def _is_fold_padding(padding) -> bool:
+    return isinstance(padding, Mapping) and "fold" in padding
+
+
+def _position_kind(position: str) -> str:
+    return "center" if position == "center" else "edge"
+
+
+def _parse_fold_padding(padding: Mapping) -> Dict:
+    """Validate a fold spec ``{"fold": pivot, "south": mode}``; returns it normalised (south defaults to fill)."""
+    if not _is_fold_padding(padding):
+        raise ValueError(f"Not a fold padding value: {padding!r}")
+    extra = set(padding) - {"fold", "south"}
+    if extra:
+        raise ValueError(
+            f"Unknown keys {sorted(extra)} in fold padding {dict(padding)!r}. "
+            "Allowed keys are 'fold' (pivot type) and 'south' (south-edge mode)."
+        )
+    pivot = padding["fold"]
+    if isinstance(pivot, str):
+        if pivot.lower() not in _PIVOT_ALIASES:
+            raise ValueError(
+                f"Unknown fold pivot {pivot!r}. Use one of {sorted(_PIVOT_ALIASES)} "
+                "or an explicit {axis: position} mapping."
+            )
+    elif isinstance(pivot, Mapping):
+        if not pivot:
+            raise ValueError("Explicit fold pivot mapping must not be empty.")
+        bad = {ax: pos for ax, pos in pivot.items() if pos not in _SEAM_POSITION}
+        if bad:
+            raise ValueError(
+                f"Invalid position(s) {bad} in explicit fold pivot {dict(pivot)!r}. "
+                f"Each must be one of {sorted(_SEAM_POSITION)}."
+            )
+    else:
+        raise ValueError(
+            f"Fold pivot must be a name ({sorted(_PIVOT_ALIASES)}) or an {{axis: position}} mapping, got {pivot!r}."
+        )
+    south = padding.get("south", "fill")
+    if south not in _XGCM_BOUNDARY_KWARG_TO_XARRAY_PAD_KWARG:
+        raise ValueError(
+            f"Fold 'south' mode must be one of {list(_XGCM_BOUNDARY_KWARG_TO_XARRAY_PAD_KWARG)}, got {south!r}."
+        )
+    return {"fold": pivot, "south": south}
+
+
+def _resolve_pivot(pivot, fold_axis: str, seam_axis: str) -> Dict[str, str]:
+    """``{"seam": center|edge, "fold": center|edge}`` of an alias or an ``{axis: position}`` mapping."""
+    if isinstance(pivot, str):
+        return dict(_PIVOT_ALIASES[pivot.lower()])
+    roles = {}
+    for axname, position in pivot.items():
+        if axname == fold_axis:
+            roles["fold"] = _position_kind(position)
+        elif axname == seam_axis:
+            roles["seam"] = _position_kind(position)
+        else:
+            raise ValueError(
+                f"Fold pivot axis {axname!r} is neither the fold axis {fold_axis!r} nor the seam axis {seam_axis!r}."
+            )
+    roles.setdefault("seam", "center")
+    roles.setdefault("fold", "center")
+    return roles
+
+
+def fold_edges(grid, ax_name: str, ax_padding, hi: int):
+    """How an axis is padded with respect to a north fold: ``(north folds, boundary mode of the other edges)``.
+
+    On a fold axis the north edge folds whenever it is padded (``hi > 0``), whatever the per-call
+    ``padding`` says; a per-call string only sets the south edge, which otherwise takes the spec's
+    ``south`` mode (reference padding.py:744-757).  Every fast path that picks itself from the padding
+    value asks this first.  Other axes: ``(False, ax_padding)``."""
+    info = grid._folds.get(ax_name)
+    if info is None:
+        return False, ax_padding
+    return hi > 0, (ax_padding if isinstance(ax_padding, str) else info["south"])
+
+
+def _fold_plan(grid, fold_axis: str, dims, shape, width: int):
+    """(fold dim number, seam dim number, skip, mirror, period) of the north halo of a field with ``dims``."""
+    info = grid._folds[fold_axis]
+    seam_axis = info["seam_axis"]
+    roles = _resolve_pivot(info["pivot"], fold_axis, seam_axis)
+    probe = DataArray.__new__(DataArray)
+    probe._dims = tuple(dims)
+    fold_pos, fold_dim = grid.axes[fold_axis]._get_position_name(probe)
+    seam_pos, seam_dim = grid.axes[seam_axis]._get_position_name(probe)
+    f, s = dims.index(fold_dim), dims.index(seam_dim)
+    n = int(shape[f])
+    skip = 1 if _position_kind(fold_pos) == roles["fold"] else 0
+    if width > n - skip:
+        raise ValueError(
+            f"North-fold halo width {width} requested on fold axis {fold_axis!r} exceeds the {n - skip} "
+            f"interior row(s) available to mirror along {fold_dim!r} (grid length {n}"
+            f"{', minus 1 redundant pole row' if skip else ''})."
+        )
+    two_off, extra = _SEAM_POSITION[seam_pos]
+    length = int(shape[s])
+    period = length + extra
+    mirror = (0 if roles["seam"] == "edge" else 1) - two_off
+    # a partner >= length exists only when period > length (inner), hit by k = (mirror - length) mod period
+    if period > length and (mirror - length) % period < length:
+        raise NotImplementedError(
+            f"A {seam_pos!r} seam position is incompatible with a center-type fold pivot (seam role "
+            f"{roles['seam']!r}): the mirror about a cell-center pole has no partner on this sublattice. "
+            "Use an edge-type pivot, or a center/left/right/outer seam position."
+        )
+    return f, s, skip, mirror, period
+
+
+def fold_halo_plane(grid, fold_axis: str, dims, x, pre=None, negate: bool = False):
+    """The folded north row of the device tensor ``x`` (dims ``dims``) as a halo plane for ``xg_stencil2``:
+    ``x``'s shape with length 1 along the fold dim, ``x * pre`` read at the mirrored cell, sign-flipped
+    for vector components.  One ``xg_fold_rows`` launch."""
+    from . import ops
+
+    f, s, skip, mirror, period = _fold_plan(grid, fold_axis, tuple(dims), list(x.shape), 1)
+    return ops.fold_rows(x, f, s, 1, skip, mirror, period, negate=negate, pre=pre)
+
+
+def _pad_fold(data, grid, padding_width, padding, fill_value):
+    """Padding on a grid with a north fold (reference padding.py:687-762), on the device.
+
+    Same order as the reference: the fold halo first, built from the unpadded field (so the seam
+    mirror sees the whole periodic row), then the south edge of the fold axis and every other axis
+    with the ordinary boundary conditions, on the array that already holds the fold rows — a
+    periodic south edge therefore wraps the fold row, and a seam padded in the same call wraps the
+    folded rows.  A vector component ``{axis: da}`` changes sign across the fold; it needs no
+    partner component (the fold is a point reflection, not a rotation)."""
+    from . import ops
+    from .device import as_device_tensor, result_like
+
+    if isinstance(data, dict):
+        isvector = True
+        [da] = list(data.values())
+    else:
+        isvector, da = False, data
+    fold_axes = [ax for ax in padding_width if ax in grid._folds and padding_width[ax][1] > 0]
+    if len(fold_axes) > 1:
+        raise NotImplementedError(
+            f"Padding more than one north-fold axis at once is not supported (got fold axes {sorted(fold_axes)})."
+        )
+    for fax in fold_axes:
+        width = int(padding_width[fax][1])
+        dims = tuple(da.dims)
+        x, was_host = as_device_tensor(da.data, grid._device_for(da))
+        f, s, skip, mirror, period = _fold_plan(grid, fax, dims, list(x.shape), width)
+        n = int(x.shape[f])
+        out = ops.pad(x, f, 0, width, "fill", 0.0)
+        ops.fold_rows(x, f, s, width, skip, mirror, period, negate=isvector, out=out, row0=n)
+        da = DataArray(result_like(out, was_host), dims=dims, name=da.name, attrs=da.attrs)
+    basic_width, basic_padding = {}, {}
+    for ax, widths in padding_width.items():
+        if ax in grid._folds:
+            basic_width[ax] = (widths[0], 0)
+            basic_padding[ax] = fold_edges(grid, ax, padding[ax], 0)[1]
+        else:
+            basic_width[ax] = widths
+            basic_padding[ax] = padding[ax]
+    return _pad_basic(da, grid, basic_width, basic_padding, fill_value)
 
 
 def _strip_all_coords(data):
@@ -54,8 +239,6 @@ def _pad_basic(da: DataArray, grid, padding_width, padding, fill_value):
                 f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
                 f"grid method."
             )
-        if isinstance(ax_padding, Mapping):
-            raise NotImplementedError("fold padding is outside the scope of xgcm_b200")
         x, was_host = as_device_tensor(out.data, grid._device_for(out))
         fv = fill_value[ax] if fill_value[ax] is not None else 0.0
         y = ops.pad(x, out.get_axis_num(dim), int(widths[0]), int(widths[1]), ax_padding, fv)
@@ -600,6 +783,8 @@ def pad(
         return _pad_face_connections(
             data, grid, padding_width, padding, fill_value, other_component=other_component
         )
+    if grid._folds and any(ax in grid._folds for ax in padding_width):
+        return _pad_fold(data, grid, padding_width, padding, fill_value)
     if isinstance(data, dict):
         [data] = list(data.values())
     return _pad_basic(data, grid, padding_width, padding, fill_value)
