@@ -195,6 +195,96 @@ def test_wreduce_rows_and_mean(dtype, rtol):
     assert np.isnan(got).all()  # xarray weighted mean: 0/0 -> NaN
 
 
+@pytest.mark.parametrize("dtype", [np.float32, np.float64])
+def test_wreduce_rows_vector_and_scalar_loads(dtype):
+    """The innermost-axis reduction reads 16-byte vectors when the rows allow it, else single elements."""
+    from xgcm_b200 import _capi, ops
+
+    rtol = 1e-6 if dtype == np.float32 else 1e-12
+    for n, side in ((1000, "vec"), (999, "scalar")):
+        a = _field((7, 9, n), dtype, seed=21, nan_frac=0.02)
+        w = (0.5 + np.random.default_rng(22).random((1, 1, n))).astype(dtype)
+        for mode in ("sum", "mean"):
+            got = ops.wreduce(_t(a), 2, _t(w), mode, True).cpu().numpy()
+            assert _capi.last_launch() == f"xg_wreduce(rows, {side})"
+            np.testing.assert_allclose(got, oracle.wreduce(a, w, 2, mode, True), rtol=rtol * 4, equal_nan=True)
+
+
+# ----------------------------------------------------------------------------- strided scan / reduce at the 16-byte switch
+# k_scan_strided and k_reduce_strided read 16-byte column vectors only from outer x inner / VEC >= XG_SMS x 64 = 8448
+# vector columns on (xg_cumscan.cu scan_launch, xg_wreduce.cu reduce_launch); below that, one element per thread.
+# Shapes exactly at the switch and just below it, along Z and along Y.
+VEC_COLUMNS = 132 * 64
+STRIDED_SWITCH = {
+    np.float32: [((40, 48, 704), 0, "vec"), ((40, 48, 700), 0, "scalar"), ((22, 30, 1536), 1, "vec"),
+                 ((22, 30, 1524), 1, "scalar")],
+    np.float64: [((40, 24, 704), 0, "vec"), ((40, 24, 700), 0, "scalar"), ((22, 30, 768), 1, "vec"),
+                 ((22, 30, 762), 1, "scalar")],
+}
+SWITCH_CASES = [(dt, shape, axis, side) for dt, cases in STRIDED_SWITCH.items() for shape, axis, side in cases]
+
+
+def _vector_columns(shape, axis, dtype):
+    vec = 16 // np.dtype(dtype).itemsize
+    return int(np.prod(shape[:axis])) * (int(np.prod(shape[axis + 1:])) // vec)
+
+
+def _switch_field(shape, dtype, seed):
+    """Uniform values with 3 % NaN and a few +-inf and -0."""
+    rng = np.random.default_rng(seed)
+    a = (rng.random(shape) - 0.25).astype(dtype)
+    r = rng.random(shape)
+    a[r < 0.03] = np.nan
+    a[(r >= 0.03) & (r < 0.031)] = np.inf
+    a[(r >= 0.031) & (r < 0.032)] = -np.inf
+    a[(r >= 0.032) & (r < 0.04)] = -0.0
+    return a
+
+
+@pytest.mark.parametrize("dtype,shape,axis,side", SWITCH_CASES)
+def test_cumscan_strided_at_vector_switch(dtype, shape, axis, side):
+    """Bit-exact cumsum either side of the switch: every trim / pad entry and boundary, reverse, skipna both ways,
+    pre-metrics shared along the axis or full, post-metrics per level along the axis or shared."""
+    from xgcm_b200 import _capi, ops
+
+    assert (_vector_columns(shape, axis, dtype) >= VEC_COLUMNS) == (side == "vec")
+    a = _switch_field(shape, dtype, 40)
+    rng = np.random.default_rng(41)
+    pres = [None, (1.0 + rng.random((1,) + shape[1:])).astype(dtype), (0.5 + rng.random(shape)).astype(dtype)]
+    k = 0
+    for (rev, trim, plo, phi), (bc, fill) in itertools.product(_cumscan_cases(), BCS):
+        oshape = list(shape)
+        oshape[axis] = shape[axis] - (0 if trim == "none" else 1) + plo + phi
+        level = [n if d == axis else 1 for d, n in enumerate(oshape)]
+        posts = [None, (1.0 + rng.random(level)).astype(dtype), (1.0 + rng.random([1] + oshape[1:])).astype(dtype)]
+        pre, post, skipna = pres[k % 3], posts[(k // 3) % 3], k % 2 == 0
+        k += 1
+        with np.errstate(invalid="ignore"):
+            want = oracle.cumscan(a, axis, rev, trim, plo, phi, bc if (plo or phi) else None, fill, pre, post, skipna)
+        got = ops.cumscan(_t(a), axis, rev, trim, plo, phi, bc, fill, _t(pre), _t(post), skipna).cpu().numpy()
+        assert _capi.last_launch() == f"xg_cumscan(strided, {side})"
+        np.testing.assert_array_equal(got, want, err_msg=f"rev={rev} trim={trim} pad=({plo},{phi}) bc={bc} skipna={skipna}")
+
+
+@pytest.mark.parametrize("dtype,shape,axis,side", SWITCH_CASES)
+def test_wreduce_strided_at_vector_switch(dtype, shape, axis, side):
+    """Bit-exact weighted sum and mean either side of the switch: no, full, (1, Y, X) and per-level weights,
+    skipna both ways."""
+    from xgcm_b200 import _capi, ops
+
+    assert (_vector_columns(shape, axis, dtype) >= VEC_COLUMNS) == (side == "vec")
+    a = _switch_field(shape, dtype, 42)
+    rng = np.random.default_rng(43)
+    level = [n if d == axis else 1 for d, n in enumerate(shape)]
+    for wshape, mode, skipna in itertools.product((None, shape, (1,) + shape[1:], level), ("sum", "mean"), (True, False)):
+        w = None if wshape is None else (0.5 + rng.random(wshape)).astype(dtype)
+        with np.errstate(invalid="ignore"):
+            want = oracle.wreduce(a, w, axis, mode, skipna)
+        got = ops.wreduce(_t(a), axis, _t(w), mode, skipna).cpu().numpy()
+        assert _capi.last_launch() == f"xg_wreduce(strided, {side})"
+        np.testing.assert_array_equal(got, want, err_msg=f"w={wshape} {mode} skipna={skipna}")
+
+
 # ----------------------------------------------------------------------------- vinterp
 def _theta_field(shape, axis, dtype, rng, decreasing_frac=0.3, nan_frac=0.0):
     n = shape[axis]

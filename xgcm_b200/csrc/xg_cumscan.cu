@@ -541,7 +541,7 @@ int scan_launch(ScanArgs<T>& a, cudaStream_t st) {
       if (blocks > 0x7fffffffLL) return xg_fail(XG_EINVAL, "xg_cumscan: grid too large");
       k_scan_strided<T, 1, MET, U><<<(unsigned)blocks, kThreads, 0, st>>>(a);
     }
-    return xg_check_launch("xg_cumscan(strided)");
+    return xg_check_launch(vec_ok ? "xg_cumscan(strided, vec)" : "xg_cumscan(strided, scalar)");
   }
   const int64_t units = xg_ceil_div(a.outer, kTile);
   constexpr int E = 16 / sizeof(T);

@@ -146,15 +146,16 @@ int reduce_launch(ReduceArgs<T>& a, cudaStream_t st) {
       k_reduce_strided<T, VEC, HASW, U><<<(unsigned)blocks, kThreads, 0, st>>>(a);
     else
       k_reduce_strided<T, 1, HASW, U><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-    return xg_check_launch("xg_wreduce(strided)");
+    return xg_check_launch(vec_ok ? "xg_wreduce(strided, vec)" : "xg_wreduce(strided, scalar)");
   }
   const int64_t blocks = xg_ceil_div(a.outer, kThreads / 32);
   if (blocks > 0x7fffffffLL) return xg_fail(XG_EINVAL, "xg_wreduce: grid too large");
-  if (a.n % VEC == 0 && ((uintptr_t)a.in & 15) == 0)
+  const bool row_vec = a.n % VEC == 0 && ((uintptr_t)a.in & 15) == 0;
+  if (row_vec)
     k_reduce_rows<T, HASW, VEC><<<(unsigned)blocks, kThreads, 0, st>>>(a);
   else
     k_reduce_rows<T, HASW, 1><<<(unsigned)blocks, kThreads, 0, st>>>(a);
-  return xg_check_launch("xg_wreduce(rows)");
+  return xg_check_launch(row_vec ? "xg_wreduce(rows, vec)" : "xg_wreduce(rows, scalar)");
 }
 
 template <typename T>
