@@ -307,6 +307,45 @@ XG_API int xg_stencil2_host(int op, int dtype, const void* in, void* out, int nd
                      const int64_t* post_strides, int device);
 
 /*
+ * xg_stencil2_host on the two grid topologies whose halo is not a boundary condition.  Same slab
+ * pipeline (workspace, slots, events, slab size), plus a per-slab halo stage on the kernel stream that
+ * builds the slab's halo_lo / halo_hi planes before its xg_stencil2 launch.  Dim 0 is cut into slabs and
+ * must be a batch dim: not the operated, fold, seam or face dim (XG_EINVAL).  Every argument is
+ * checked before any CUDA call.
+ *
+ * _fold: north fold along `axis` (hi must be 1).  Per slab, one xg_fold_rows launch (width 1; seam_axis,
+ * skip, mirror, period, negate as there, `pre_metric` read at the mirrored cell) writes halo_hi; with
+ * lo = 1 and bc = XG_BC_PERIODIC it is halo_lo too, any other bc pads the south edge as usual.
+ * XG_ENOTIMPL where xg_fold_rows would return it.
+ *
+ * _connected: face connections.  The halo planes (the field's shape with extent 1 along `axis`) are
+ * written by `ncopies` strided copies of rank `copy_ndim` (copy k: side[k] 0 = lo plane, 1 = hi plane;
+ * source[k] 0 = the field, 1 = `partner`, the other component of a vector, 2 = the constant fill_value;
+ * element offsets into plane and source, then shape, strides and negate as in xg_strided_copy_batch),
+ * described once for the WHOLE field: every copy spans dim 0 in full from index 0, with the contiguous
+ * dim-0 strides of the plane and of its source (0 for the constant).  The copies must write disjoint
+ * cells that cover each padded plane.  `partner` (optional, shape `partner_shape`, same ndim and dim-0
+ * extent as the field) is streamed slab by slab beside it.  No pre-metric.
+ */
+XG_API int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
+                                 const int64_t* shape, int axis, int lo, int hi, int bc,
+                                 double fill_value, const void* pre_metric, const int64_t* pre_strides,
+                                 const void* post_metric, const int64_t* post_strides, int seam_axis,
+                                 int skip, int64_t mirror, int64_t period, int negate, int device);
+XG_API int xg_stencil2_host_connected(int op, int dtype, const void* in, const void* partner,
+                                      const int64_t* partner_shape, void* out, int ndim,
+                                      const int64_t* shape, int axis, int lo, int hi, double fill_value,
+                                      const void* post_metric, const int64_t* post_strides, int ncopies,
+                                      int copy_ndim, const int* side, const int* source,
+                                      const int64_t* dst_offset, const int64_t* src_offset,
+                                      const int64_t* shapes, const int64_t* dst_strides,
+                                      const int64_t* src_strides, const int* negate, int device);
+
+/* Device bytes the workspace of xg_stencil2_host and its _fold / _connected variants holds on `device`
+ * (slot buffers, metrics, halo planes); 0 before the first call or after xg_host_workspace_release. */
+XG_API int xg_host_workspace_bytes(int device, int64_t* bytes);
+
+/*
  * One HOST field up, `nout` results down: result k = xg_stencil2(op[k], axis[k], lo[k], hi[k], bc[k],
  * fill_value[k]) of the same input (no metrics), each into its own HOST buffer out[k].  The field crosses
  * PCIe once instead of once per result (the reference re-reads it per call, xgcm/grid.py:796-832).

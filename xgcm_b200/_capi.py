@@ -88,6 +88,17 @@ SIGNATURES = {
         [C.c_int, C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int,
          C.c_double, _vp, _i64p, _vp, _i64p, C.c_int],
     ),
+    "xg_stencil2_host_fold": (
+        C.c_int,
+        [C.c_int, C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int,
+         C.c_double, _vp, _i64p, _vp, _i64p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int],
+    ),
+    "xg_stencil2_host_connected": (
+        C.c_int,
+        [C.c_int, C.c_int, _vp, _vp, _i64p, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_double,
+         _vp, _i64p, C.c_int, C.c_int, _i32p, _i32p, _i64p, _i64p, _i64p, _i64p, _i64p, _i32p, C.c_int],
+    ),
+    "xg_host_workspace_bytes": (C.c_int, [C.c_int, _i64p]),
     "xg_stencil2_host_multi": (
         C.c_int,
         [C.c_int, _i32p, C.c_int, _vp, _vpp, C.c_int, _i64p, _i32p, _i32p, _i32p, _i32p, _f64p, C.c_int],

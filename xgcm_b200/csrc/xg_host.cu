@@ -9,6 +9,12 @@
 // When dim 0 is the operated axis the slabs overlap by the one-cell halo and the
 // exterior halo plane (periodic wrap) is uploaded once.
 //
+// xg_stencil2_host_fold / xg_stencil2_host_connected run the same slab loop with a per-slab halo stage
+// on the kernel stream: the slab's halo_lo / halo_hi planes are built from the slab buffers (one
+// xg_fold_rows launch, or the face-connection copy list clipped to the slab and replayed with
+// xg_strided_copy_batch) just before its xg_stencil2 launch.  Dim 0 is then a batch dim, so the planes
+// of one slab depend on that slab (and the partner component's slab) alone.
+//
 // Workspace (device slabs + events + streams) is cached per device and reused;
 // xg_host_workspace_release() frees it.
 #include <stdlib.h>
@@ -26,10 +32,13 @@ struct Workspace {
   int device = -1;
   std::mutex mu;  // one host call at a time per device; different devices run concurrently
   size_t slab_in_bytes = 0, slab_out_bytes = 0, metric_bytes[2] = {0, 0}, halo_bytes = 0;
+  size_t partner_bytes = 0, const_bytes = 0;
   void* d_in[kSlots] = {nullptr, nullptr, nullptr};
   void* d_out[kSlots] = {nullptr, nullptr, nullptr};
+  void* d_partner[kSlots] = {nullptr, nullptr, nullptr};  // second vector component (face connections)
   void* d_metric[2] = {nullptr, nullptr};
-  void* d_halo[2] = {nullptr, nullptr};
+  void* d_halo[2] = {nullptr, nullptr};  // wrap planes along dim 0, or the per-slab lo / hi halo planes
+  void* d_const = nullptr;               // the fill constant the unconnected face edges copy from
   cudaStream_t s_h2d = nullptr, s_k = nullptr, s_d2h = nullptr;
   cudaEvent_t e_up[kSlots], e_done[kSlots], e_down[kSlots];
   bool events = false;
@@ -98,6 +107,7 @@ extern "C" int xg_host_workspace_release(void) {
     for (int i = 0; i < kSlots; ++i) {
       if (w->d_in[i]) cudaFree(w->d_in[i]);
       if (w->d_out[i]) cudaFree(w->d_out[i]);
+      if (w->d_partner[i]) cudaFree(w->d_partner[i]);
       if (w->events) {
         cudaEventDestroy(w->e_up[i]);
         cudaEventDestroy(w->e_done[i]);
@@ -108,6 +118,7 @@ extern "C" int xg_host_workspace_release(void) {
       if (w->d_metric[i]) cudaFree(w->d_metric[i]);
       if (w->d_halo[i]) cudaFree(w->d_halo[i]);
     }
+    if (w->d_const) cudaFree(w->d_const);
     if (w->s_h2d) cudaStreamDestroy(w->s_h2d);
     if (w->s_k) cudaStreamDestroy(w->s_k);
     if (w->s_d2h) cudaStreamDestroy(w->s_d2h);
@@ -117,29 +128,107 @@ extern "C" int xg_host_workspace_release(void) {
   return XG_OK;
 }
 
-extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, int ndim,
-                                const int64_t* shape, int axis, int lo, int hi, int bc,
-                                double fill_value, const void* pre_metric,
-                                const int64_t* pre_strides, const void* post_metric,
-                                const int64_t* post_strides, int device) {
-  if (!in || !out || !shape) return xg_fail(XG_EINVAL, "xg_stencil2_host: null pointer");
-  if (dtype != XG_F32 && dtype != XG_F64)
-    return xg_fail(XG_EINVAL, "xg_stencil2_host: dtype must be XG_F32 or XG_F64");
-  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, "xg_stencil2_host: bad ndim");
-  if (axis < 0 || axis >= ndim) return xg_fail(XG_EINVAL, "xg_stencil2_host: axis out of range");
-  if (lo < 0 || lo > 1 || hi < 0 || hi > 1)
-    return xg_fail(XG_EINVAL, "xg_stencil2_host: halo widths must be 0 or 1");
-  if ((lo || hi) && (bc <= XG_BC_NONE || bc > XG_BC_EXTRAPOLATE))
-    return xg_fail(XG_EINVAL,
-                   "xg_stencil2_host: no boundary condition was specified but the operation "
-                   "needs to pad the axis");
-  const size_t es = dtype == XG_F32 ? 4 : 8;
-  XG_CUDA(cudaSetDevice(device));
+namespace {
+
+// The stencil call the slab loop runs, slab by slab.
+struct Call {
+  int op, dtype;
+  const void* in;
+  void* out;
+  int ndim;
+  const int64_t* shape;
+  int axis, lo, hi, bc;
+  double fill_value;
+  const void* pre;
+  const int64_t* pre_strides;
+  const void* post;
+  const int64_t* post_strides;
+  int device;
+};
+
+enum { kHaloNone = 0, kHaloFold = 1, kHaloCopies = 2 };
+enum { kSrcField = 0, kSrcPartner = 1, kSrcFill = 2 };
+
+// What builds a slab's halo planes on s_k before its xg_stencil2 launch (none for xg_stencil2_host).
+struct HaloStage {
+  int kind = kHaloNone;
+  // kHaloFold: the folded north row of the slab is halo_hi, and halo_lo when the south edge is periodic
+  int seam_axis = 0, skip = 0, negate = 0;
+  int64_t mirror = 0, period = 1;
+  // kHaloCopies: strided copies into the lo / hi planes, described once for the whole field (dim-0 extent n0)
+  const void* partner = nullptr;
+  int64_t partner_row = 0;  // partner elements per dim-0 index
+  int ncopies = 0, cndim = 0;
+  const int *side = nullptr, *source = nullptr, *negate_c = nullptr;
+  const int64_t *dst_offset = nullptr, *src_offset = nullptr, *shapes = nullptr;
+  const int64_t *dst_strides = nullptr, *src_strides = nullptr;
+};
+
+// Argument checks shared by the host stencil entry points; no CUDA call.
+int validate_call(const char* who, const Call& c) {
+  const std::string w(who);
+  if (!c.in || !c.out || !c.shape) return xg_fail(XG_EINVAL, w + ": null pointer");
+  if (c.dtype != XG_F32 && c.dtype != XG_F64)
+    return xg_fail(XG_EINVAL, w + ": dtype must be XG_F32 or XG_F64");
+  if (c.ndim < 1 || c.ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, w + ": bad ndim");
+  if (c.axis < 0 || c.axis >= c.ndim) return xg_fail(XG_EINVAL, w + ": axis out of range");
+  if (c.lo < 0 || c.lo > 1 || c.hi < 0 || c.hi > 1)
+    return xg_fail(XG_EINVAL, w + ": halo widths must be 0 or 1");
+  if ((c.lo || c.hi) && (c.bc <= XG_BC_NONE || c.bc > XG_BC_EXTRAPOLATE))
+    return xg_fail(XG_EINVAL, w + ": no boundary condition was specified but the operation needs to pad the axis");
+  if (c.shape[c.axis] == 0) return xg_fail(XG_EINVAL, w + ": empty operated axis");
+  if ((c.pre && !c.pre_strides) || (c.post && !c.post_strides))
+    return xg_fail(XG_EINVAL, w + ": metric strides missing");
+  if (c.axis == 0 && c.bc == XG_BC_PERIODIC && c.pre)
+    return xg_fail(XG_ENOTIMPL, w + ": periodic halo with a pre-metric along the outermost axis; "
+                                    "use the device entry point");
+  return XG_OK;
+}
+
+// The halo entry points build their planes per slab: dim 0 must be a batch dim the halo does not touch.
+int validate_halo_call(const char* who, const Call& c) {
+  int rc = validate_call(who, c);
+  if (rc) return rc;
+  if (c.ndim < 2 || c.axis == 0)
+    return xg_fail(XG_EINVAL, std::string(who) + ": dim 0 is cut into slabs and must not be the operated dim");
+  for (int d = 0; d < c.ndim; ++d)
+    if (c.shape[d] < 0) return xg_fail(XG_EINVAL, std::string(who) + ": negative extent");
+  return XG_OK;
+}
+
+// Per-slab face-connection copies: rebase the whole-field copy list onto the slab buffers, `rows` high.
+int halo_copies(const HaloStage& h, int dtype, size_t es, void* const planes[2], const void* field,
+                const void* partner, const void* fill, int64_t rows, std::vector<void*>& dptr,
+                std::vector<const void*>& sptr, std::vector<int64_t>& shp, cudaStream_t st) {
+  for (int k = 0; k < h.ncopies; ++k) {
+    dptr[k] = (char*)planes[h.side[k]] + (size_t)h.dst_offset[k] * es;
+    const void* base = h.source[k] == kSrcField ? field : h.source[k] == kSrcPartner ? partner : fill;
+    sptr[k] = (const char*)base + (size_t)h.src_offset[k] * es;
+    shp[(size_t)k * h.cndim] = rows;
+  }
+  int rc = xg_strided_copy_batch(dtype, h.ncopies, dptr.data(), sptr.data(), h.cndim, shp.data(),
+                                 h.dst_strides, h.src_strides, h.negate_c, st);
+  if (rc != XG_ENOTIMPL) return rc;
+  for (int k = 0; k < h.ncopies; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
+    rc = xg_strided_copy(dtype, dptr[k], h.dst_strides + (size_t)k * h.cndim, sptr[k],
+                         h.src_strides + (size_t)k * h.cndim, h.cndim, shp.data() + (size_t)k * h.cndim,
+                         h.negate_c[k], st);
+    if (rc) return rc;
+  }
+  return XG_OK;
+}
+
+// The slab loop of every host stencil entry point (arguments already validated).
+int run_slabs(const Call& c, const HaloStage& h) {
+  const int ndim = c.ndim, axis = c.axis, lo = c.lo, hi = c.hi, bc = c.bc;
+  const int64_t* shape = c.shape;
+  const size_t es = c.dtype == XG_F32 ? 4 : 8;
+  XG_CUDA(cudaSetDevice(c.device));
   Workspace* w = nullptr;
   int rc;
   {
     std::lock_guard<std::mutex> reg(g_ws_mutex);  // registry only
-    rc = get_workspace(device, &w);
+    rc = get_workspace(c.device, &w);
   }
   if (rc) return rc;
   std::lock_guard<std::mutex> lock(w->mu);
@@ -147,7 +236,6 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
   int64_t out_shape[XG_MAX_NDIM];
   for (int d = 0; d < ndim; ++d) out_shape[d] = shape[d];
   out_shape[axis] = shape[axis] + lo + hi - 1;
-  if (shape[axis] == 0) return xg_fail(XG_EINVAL, "xg_stencil2_host: empty operated axis");
   int64_t row_in = 1, row_out = 1;  // elements per index of dim 0
   for (int d = 1; d < ndim; ++d) {
     row_in *= shape[d];
@@ -178,38 +266,38 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
   const int64_t in_rows_max = ax0 ? rows + 1 : rows;
 
   for (int i = 0; i < kSlots; ++i) {
-    size_t have_in = w->slab_in_bytes, have_out = w->slab_out_bytes;
+    size_t have_in = w->slab_in_bytes, have_out = w->slab_out_bytes, have_p = w->partner_bytes;
     rc = ensure(&w->d_in[i], &have_in, (size_t)(in_rows_max * row_in) * es);
     if (rc) return rc;
     rc = ensure(&w->d_out[i], &have_out, (size_t)(rows * row_out) * es);
     if (rc) return rc;
+    if (h.partner) {
+      rc = ensure(&w->d_partner[i], &have_p, (size_t)(rows * h.partner_row) * es);
+      if (rc) return rc;
+    }
     if (i == kSlots - 1) {
       w->slab_in_bytes = have_in;
       w->slab_out_bytes = have_out;
+      w->partner_bytes = have_p;
     }
   }
   // (all three slots share one recorded capacity: grow them together)
   // metrics: uploaded whole, once
-  const void* hm[2] = {pre_metric, post_metric};
-  const int64_t* ms[2] = {pre_strides, post_strides};
+  const void* hm[2] = {c.pre, c.post};
+  const int64_t* ms[2] = {c.pre_strides, c.post_strides};
   const int64_t* mshape[2] = {shape, out_shape};
   for (int k = 0; k < 2; ++k) {
     if (!hm[k]) continue;
-    if (!ms[k]) return xg_fail(XG_EINVAL, "xg_stencil2_host: metric strides missing");
     const size_t span = operand_span(ms[k], mshape[k], ndim, es);
     rc = ensure(&w->d_metric[k], &w->metric_bytes[k], span);
     if (rc) return rc;
     XG_CUDA(cudaMemcpyAsync(w->d_metric[k], hm[k], span, cudaMemcpyHostToDevice, w->s_h2d));
   }
   // exterior halo planes when dim 0 is the operated axis and the halo is data (periodic wrap)
-  const char* hin = static_cast<const char*>(in);
-  char* hout = static_cast<char*>(out);
+  const char* hin = static_cast<const char*>(c.in);
+  char* hout = static_cast<char*>(c.out);
   const int64_t n0 = shape[0];
-  bool wrap_planes = ax0 && bc == XG_BC_PERIODIC && (pre_metric == nullptr);
-  if (ax0 && bc == XG_BC_PERIODIC && pre_metric != nullptr)
-    return xg_fail(XG_ENOTIMPL,
-                   "xg_stencil2_host: periodic halo with a pre-metric along the outermost axis; "
-                   "use the device entry point");
+  const bool wrap_planes = ax0 && bc == XG_BC_PERIODIC && c.pre == nullptr;
   if (wrap_planes) {
     size_t hb = w->halo_bytes;
     for (int k = 0; k < 2; ++k) {
@@ -223,6 +311,30 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
                               cudaMemcpyHostToDevice, w->s_h2d));
     if (hi)
       XG_CUDA(cudaMemcpyAsync(w->d_halo[1], hin, row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
+  }
+  // per-slab halo planes (dim 0 is not the operated axis): one pair, built and read in order on s_k
+  std::vector<void*> dptr(h.ncopies);
+  std::vector<const void*> sptr(h.ncopies);
+  std::vector<int64_t> shp(h.shapes ? h.shapes : (const int64_t*)nullptr,
+                           h.shapes ? h.shapes + (size_t)h.ncopies * h.cndim : (const int64_t*)nullptr);
+  if (h.kind != kHaloNone) {
+    const int64_t plane_row = row_in / shape[axis];
+    size_t hb = w->halo_bytes;
+    for (int k = 0; k < 2; ++k) {
+      size_t have = hb;
+      rc = ensure(&w->d_halo[k], &have, (size_t)(rows * plane_row) * es);
+      if (rc) return rc;
+      if (k == 1) w->halo_bytes = have;
+    }
+    bool fill = false;
+    for (int k = 0; k < h.ncopies; ++k) fill = fill || h.source[k] == kSrcFill;
+    if (fill) {
+      rc = ensure(&w->d_const, &w->const_bytes, es);
+      if (rc) return rc;
+      const float f32 = (float)c.fill_value;  // pageable: staged before cudaMemcpyAsync returns
+      XG_CUDA(cudaMemcpyAsync(w->d_const, es == 4 ? (const void*)&f32 : (const void*)&c.fill_value, es,
+                              cudaMemcpyHostToDevice, w->s_h2d));
+    }
   }
   XG_CUDA(cudaEventRecord(w->e_up[0], w->s_h2d));
   XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[0], 0));  // metrics + halo planes before any kernel
@@ -266,6 +378,10 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
       XG_CUDA(cudaMemcpyAsync(w->d_in[slot], hin + (size_t)i0 * row_in * es,
                               (size_t)(i1 - i0) * row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
     }
+    if (h.partner)
+      XG_CUDA(cudaMemcpyAsync(w->d_partner[slot],
+                              static_cast<const char*>(h.partner) + (size_t)(i0 * h.partner_row) * es,
+                              (size_t)((i1 - i0) * h.partner_row) * es, cudaMemcpyHostToDevice, w->s_h2d));
     prev_last_row = i1 - 1;
     prev_last_ptr = (const char*)w->d_in[slot] + (size_t)(i1 - 1 - i0) * row_in * es;
     XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
@@ -274,19 +390,29 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
     slab_shape[0] = i1 - i0;
     const char* pm = (const char*)w->d_metric[0];
     const char* qm = (const char*)w->d_metric[1];
-    if (pre_metric) pm += (size_t)(i0 * pre_strides[0]) * es;
-    if (post_metric) qm += (size_t)(j0 * post_strides[0]) * es;
+    if (c.pre) pm += (size_t)(i0 * c.pre_strides[0]) * es;
+    if (c.post) qm += (size_t)(j0 * c.post_strides[0]) * es;
     const void* hl = nullptr;
     const void* hh = nullptr;
-    int slab_bc = bc;
     if (ax0 && wrap_planes) {
       if (slab_lo) hl = w->d_halo[0];
       if (slab_hi) hh = w->d_halo[1];
     }
-    rc = xg_stencil2(op, dtype, w->d_in[slot], w->d_out[slot], ndim, slab_shape, axis, slab_lo,
-                     slab_hi, (slab_lo || slab_hi) ? slab_bc : XG_BC_NONE, fill_value,
-                     pre_metric ? pm : nullptr, pre_strides, post_metric ? qm : nullptr,
-                     post_strides, hl, hh, w->s_k);
+    if (h.kind == kHaloFold) {
+      rc = xg_fold_rows(c.dtype, w->d_in[slot], w->d_halo[1], ndim, slab_shape, axis, h.seam_axis, 1, 0, 1,
+                        h.skip, h.mirror, h.period, h.negate, c.pre ? pm : nullptr, c.pre_strides, w->s_k);
+      hh = w->d_halo[1];
+      if (lo && bc == XG_BC_PERIODIC) hl = hh;  // a periodic south edge wraps the row above the top
+    } else if (h.kind == kHaloCopies) {
+      rc = halo_copies(h, c.dtype, es, w->d_halo, w->d_in[slot], w->d_partner[slot], w->d_const, i1 - i0,
+                       dptr, sptr, shp, w->s_k);
+      if (lo) hl = w->d_halo[0];
+      if (hi) hh = w->d_halo[1];
+    }
+    if (rc == XG_OK)
+      rc = xg_stencil2(c.op, c.dtype, w->d_in[slot], w->d_out[slot], ndim, slab_shape, axis, slab_lo, slab_hi,
+                       (slab_lo || slab_hi) ? bc : XG_BC_NONE, c.fill_value, c.pre ? pm : nullptr,
+                       c.pre_strides, c.post ? qm : nullptr, c.post_strides, hl, hh, w->s_k);
     if (rc) {
       cudaDeviceSynchronize();
       return rc;
@@ -300,5 +426,168 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
   XG_CUDA(cudaStreamSynchronize(w->s_d2h));
   XG_CUDA(cudaStreamSynchronize(w->s_k));
   XG_CUDA(cudaStreamSynchronize(w->s_h2d));
+  return XG_OK;
+}
+
+// lowest and highest element a strided copy of `shape` touches from `offset`
+void copy_extent(int64_t offset, const int64_t* strides, const int64_t* shape, int ndim, int64_t* lo,
+                 int64_t* hi) {
+  *lo = *hi = offset;
+  for (int d = 0; d < ndim; ++d) {
+    const int64_t span = (shape[d] - 1) * strides[d];
+    if (span < 0) *lo += span;
+    else *hi += span;
+  }
+}
+
+}  // namespace
+
+extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, int ndim,
+                                const int64_t* shape, int axis, int lo, int hi, int bc,
+                                double fill_value, const void* pre_metric,
+                                const int64_t* pre_strides, const void* post_metric,
+                                const int64_t* post_strides, int device) {
+  const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, bc, fill_value,
+               pre_metric, pre_strides, post_metric, post_strides, device};
+  int rc = validate_call("xg_stencil2_host", c);
+  if (rc) return rc;
+  return run_slabs(c, HaloStage{});
+}
+
+extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
+                                     const int64_t* shape, int axis, int lo, int hi, int bc,
+                                     double fill_value, const void* pre_metric, const int64_t* pre_strides,
+                                     const void* post_metric, const int64_t* post_strides, int seam_axis,
+                                     int skip, int64_t mirror, int64_t period, int negate, int device) {
+  const char* who = "xg_stencil2_host_fold";
+  const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, bc, fill_value,
+               pre_metric, pre_strides, post_metric, post_strides, device};
+  int rc = validate_halo_call(who, c);
+  if (rc) return rc;
+  if (seam_axis < 0 || seam_axis >= ndim) return xg_fail(XG_EINVAL, std::string(who) + ": seam axis out of range");
+  if (seam_axis == 0)
+    return xg_fail(XG_EINVAL, std::string(who) + ": dim 0 is cut into slabs and must not be the seam dim");
+  if (seam_axis == axis)
+    return xg_fail(XG_EINVAL, std::string(who) + ": the fold and seam axes must differ");
+  if (hi != 1) return xg_fail(XG_EINVAL, std::string(who) + ": the fold is the upper halo: hi must be 1");
+  if (skip < 0 || skip > 1) return xg_fail(XG_EINVAL, std::string(who) + ": skip must be 0 or 1");
+  if (shape[axis] - skip < 1)
+    return xg_fail(XG_EINVAL, std::string(who) + ": halo width exceeds the interior rows of the fold axis");
+  if (period < 1) return xg_fail(XG_EINVAL, std::string(who) + ": period must be positive");
+  for (int64_t k = 0; k < shape[seam_axis]; ++k) {  // the check xg_fold_rows makes, before any CUDA call
+    int64_t src = (mirror - k) % period;
+    if (src < 0) src += period;
+    if (src >= shape[seam_axis])
+      return xg_fail(XG_ENOTIMPL, std::string(who) + ": seam position incompatible with the pivot: the mirror "
+                                                     "partner of a seam index lies outside the seam dim");
+  }
+  HaloStage h;
+  h.kind = kHaloFold;
+  h.seam_axis = seam_axis;
+  h.skip = skip;
+  h.mirror = mirror;
+  h.period = period;
+  h.negate = negate ? 1 : 0;
+  return run_slabs(c, h);
+}
+
+extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, const void* partner,
+                                          const int64_t* partner_shape, void* out, int ndim,
+                                          const int64_t* shape, int axis, int lo, int hi, double fill_value,
+                                          const void* post_metric, const int64_t* post_strides, int ncopies,
+                                          int copy_ndim, const int* side, const int* source,
+                                          const int64_t* dst_offset, const int64_t* src_offset,
+                                          const int64_t* shapes, const int64_t* dst_strides,
+                                          const int64_t* src_strides, const int* negate, int device) {
+  const std::string who = "xg_stencil2_host_connected";
+  const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, (lo || hi) ? XG_BC_FILL : XG_BC_NONE,
+               fill_value, nullptr, nullptr, post_metric, post_strides, device};
+  int rc = validate_halo_call(who.c_str(), c);
+  if (rc) return rc;
+  if (ncopies < 0) return xg_fail(XG_EINVAL, who + ": negative copy count");
+  if (ncopies > 0 && (!side || !source || !dst_offset || !src_offset || !shapes || !dst_strides ||
+                      !src_strides || !negate))
+    return xg_fail(XG_EINVAL, who + ": null pointer in the copy list");
+  if (ncopies > 0 && (copy_ndim < 1 || copy_ndim > XG_MAX_NDIM))
+    return xg_fail(XG_EINVAL, who + ": bad copy rank");
+  if (partner && !partner_shape) return xg_fail(XG_EINVAL, who + ": null partner shape");
+  const int64_t n0 = shape[0];
+  int64_t row_in = 1;
+  for (int d = 1; d < ndim; ++d) row_in *= shape[d];
+  const int64_t plane_row = shape[axis] ? row_in / shape[axis] : 0;
+  int64_t partner_row = 0;
+  if (partner) {
+    if (partner_shape[0] != n0)
+      return xg_fail(XG_EINVAL, who + ": the partner component's dim-0 extent differs from the field's");
+    partner_row = 1;
+    for (int d = 1; d < ndim; ++d) {
+      if (partner_shape[d] < 0) return xg_fail(XG_EINVAL, who + ": negative partner extent");
+      partner_row *= partner_shape[d];
+    }
+  }
+  int64_t covered[2] = {0, 0};
+  for (int k = 0; k < ncopies; ++k) {
+    const int64_t* sh = shapes + (size_t)k * copy_ndim;
+    const int64_t* ds = dst_strides + (size_t)k * copy_ndim;
+    const int64_t* ss = src_strides + (size_t)k * copy_ndim;
+    const std::string at = who + ": copy " + std::to_string(k) + ": ";
+    if (side[k] != 0 && side[k] != 1) return xg_fail(XG_EINVAL, at + "side must be 0 (lo) or 1 (hi)");
+    if (!(side[k] ? hi : lo)) return xg_fail(XG_EINVAL, at + "writes a halo plane the call does not pad");
+    if (source[k] < kSrcField || source[k] > kSrcFill)
+      return xg_fail(XG_EINVAL, at + "source must be 0 (field), 1 (partner) or 2 (fill constant)");
+    if (source[k] == kSrcPartner && !partner) return xg_fail(XG_EINVAL, at + "reads a partner that was not given");
+    int64_t cells = 1;
+    for (int d = 0; d < copy_ndim; ++d) {
+      if (sh[d] < 0) return xg_fail(XG_EINVAL, at + "negative extent");
+      cells *= sh[d];
+    }
+    covered[side[k]] += cells;
+    const int64_t src_row = source[k] == kSrcField ? row_in : source[k] == kSrcPartner ? partner_row : 0;
+    if (sh[0] != n0 || ds[0] != plane_row || ss[0] != src_row)
+      return xg_fail(XG_EINVAL, at + "must span dim 0 in full with the contiguous dim-0 strides");
+    if (cells == 0) continue;
+    int64_t a, b;
+    copy_extent(dst_offset[k], ds, sh, copy_ndim, &a, &b);
+    if (a < 0 || b >= n0 * plane_row) return xg_fail(XG_EINVAL, at + "leaves the halo plane");
+    copy_extent(src_offset[k], ss, sh, copy_ndim, &a, &b);
+    if (source[k] == kSrcFill) {
+      if (a != 0 || b != 0) return xg_fail(XG_EINVAL, at + "the fill constant is read with offset 0, strides 0");
+    } else if (a < 0 || b >= n0 * src_row) {
+      return xg_fail(XG_EINVAL, at + "leaves its source array");
+    }
+  }
+  // the copies write disjoint cells, so together they must cover each padded plane exactly once
+  if ((lo && covered[0] != n0 * plane_row) || (hi && covered[1] != n0 * plane_row))
+    return xg_fail(XG_EINVAL, who + ": the copies do not cover the halo planes");
+  HaloStage h;
+  h.kind = kHaloCopies;
+  h.partner = partner;
+  h.partner_row = partner_row;
+  h.ncopies = ncopies;
+  h.cndim = copy_ndim;
+  h.side = side;
+  h.source = source;
+  h.negate_c = negate;
+  h.dst_offset = dst_offset;
+  h.src_offset = src_offset;
+  h.shapes = shapes;
+  h.dst_strides = dst_strides;
+  h.src_strides = src_strides;
+  return run_slabs(c, h);
+}
+
+extern "C" int xg_host_workspace_bytes(int device, int64_t* bytes) {
+  if (!bytes) return xg_fail(XG_EINVAL, "xg_host_workspace_bytes: null pointer");
+  *bytes = 0;
+  Workspace* w = nullptr;
+  {
+    std::lock_guard<std::mutex> reg(g_ws_mutex);
+    for (Workspace* x : g_ws)
+      if (x->device == device) w = x;
+  }
+  if (!w) return XG_OK;
+  std::lock_guard<std::mutex> lock(w->mu);
+  *bytes = (int64_t)(kSlots * (w->slab_in_bytes + w->slab_out_bytes + w->partner_bytes) + w->metric_bytes[0] +
+                     w->metric_bytes[1] + 2 * w->halo_bytes + w->const_bytes);
   return XG_OK;
 }

@@ -550,6 +550,10 @@ def _apply_connected_stencil(op, da, raw_arg, other_component, grid, ax_name, in
 
     lo, hi = padding_width_real.get(ax_name, (0, 0))
     if pre_metric is None and lo <= 1 and hi <= 1:
+        streamed = _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi,
+                                             padding, fill_value, post_metric_fn)
+        if streamed is not None:
+            return streamed
         # halo planes gathered from the neighbour faces, then the ordinary fused launch
         from .padding import connected_halo_planes
 
@@ -621,19 +625,36 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
     bc = ax_padding if (lo or hi) else None
     fv = fills[ax_name] if fills[ax_name] is not None else 0.0
 
-    if (not folded and not da.is_device and isinstance(da.data, np.ndarray)
-            and da.data.dtype in (np.float32, np.float64)):
-        # host field: stream slabs H2D -> kernel -> D2H inside the library (xg_stencil2_host)
-        try:
-            out = ops.stencil2_host(
-                da.data, axis_num, op, lo, hi, bc, fv,
-                pre=None if pre_metric is None else grid._metric_host(pre_metric, da.dims, da.data.dtype),
-                post=None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype),
-                device=grid._device_for(da).index,
-            )
-            return DataArray(out, dims=out_dims, name=da.name, attrs=da.attrs)
-        except NotImplementedError:
-            pass  # e.g. periodic halo + pre-metric along the outermost axis: whole-field path below
+    if _is_host_float(da) and (not folded or grid._device_for(da).type == "cuda"):
+        # host field: stream slabs H2D -> kernel -> D2H inside the library (xg_stencil2_host, or
+        # xg_stencil2_host_fold with the folded row of each slab as its north halo)
+        dims, shape = tuple(da.dims), list(da.shape)
+        pre_h = None if pre_metric is None else grid._metric_host(pre_metric, dims, da.data.dtype)
+        post_h = None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype)
+        core = [in_dim]
+        if folded:
+            from .padding import _axis_dim, _fold_plan
+
+            core.append(_axis_dim(grid, dims, grid._folds[ax_name]["seam_axis"]))
+        route = _host_stream_route("fold" if folded else "plain", dims, shape, core, lo, hi,
+                                   operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
+        if route is not None:
+            _, ndrop, nmerge = route
+            cut = lambda a: _merge_leading(a, ndrop, nmerge)  # noqa: E731
+            x = cut(da.data)
+            ax = axis_num - ndrop - nmerge + 1
+            kw = dict(pre=None if pre_h is None else cut(pre_h), post=None if post_h is None else cut(post_h),
+                      device=grid._device_for(da).index)
+            try:
+                if folded:
+                    _, seam, skip, mirror, period = _fold_plan(grid, ax_name, dims, shape, 1)
+                    out = ops.stencil2_host_fold(x, ax, op, lo, hi, bc, fv, seam - ndrop - nmerge + 1, skip, mirror,
+                                                 period, negate=isinstance(raw_arg, dict), **kw)
+                else:
+                    out = ops.stencil2_host(x, ax, op, lo, hi, bc, fv, **kw)
+                return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
+            except NotImplementedError:
+                pass  # e.g. periodic halo + pre-metric along the outermost axis: whole-field path below
 
     x, was_host = as_device_tensor(da.data, grid._device_for(da))
     pre_t = grid._metric_tensor(pre_metric, da.dims, x) if pre_metric is not None else None
@@ -647,6 +668,96 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             halo_lo = halo_hi
     out = ops.stencil2(x, axis_num, op, lo, hi, bc, fv, pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
     return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
+
+
+def _is_host_float(da) -> bool:
+    return not da.is_device and isinstance(da.data, np.ndarray) and da.data.dtype in (np.float32, np.float64)
+
+
+def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_ok=True, operand_shapes=()):
+    """Whether a numpy field streams through a host slab pipeline, and how it is cut.
+
+    ``kind``: "plain" (``xg_stencil2_host``), "fold" (the operator crosses a north fold) or "connected" (face
+    connections); ``core_dims``: the dims the operator or any halo source indexes (operated dim; seam dim;
+    face dim and the dims of the connection axes).  The slabs are cut along dim 0: leading size-1 dims are
+    dropped first, then the leading batch dims (those before the first core dim) are merged into one dim 0
+    -- as far as every broadcast operand (metric ``operand_shapes``, 1 where it broadcasts) merges with them.
+    A plain grid cuts the field's own dim 0 (no merge), which may be the operated dim.  Returns ``(kind,
+    dims dropped, dims merged)``, or None for the whole-field device path: a fold or connected field with no
+    batch dim in front, a halo wider than one cell, a pre-metric or a partner component that cannot stream
+    beside the field on a connected grid."""
+    first = min(list(dims).index(d) for d in core_dims)
+    ndrop = 0
+    while ndrop < first and shape[ndrop] == 1:
+        ndrop += 1
+    if kind == "plain":
+        return kind, ndrop, 1
+    if lo > 1 or hi > 1 or first == ndrop or (kind == "connected" and (pre or not partner_ok)):
+        return None
+    nmerge = first - ndrop
+
+    def merges(m, k):
+        sizes = [(int(a), int(b)) for a, b in zip(m[ndrop:ndrop + k], shape[ndrop:ndrop + k]) if b != 1]
+        return all(a == b for a, b in sizes) or all(a == 1 for a, _ in sizes)
+
+    while nmerge > 1 and not all(merges(m, nmerge) for m in operand_shapes):
+        nmerge -= 1
+    return kind, ndrop, nmerge
+
+
+def _merge_leading(a, ndrop, nmerge):
+    """``a`` (C-contiguous, or a metric with 1 where it broadcasts) without its first ``ndrop`` dims and with
+    the next ``nmerge`` merged into one (``_host_stream_route`` checked that this is a reshape)."""
+    a = np.ascontiguousarray(a)
+    return a.reshape((int(np.prod(a.shape[ndrop:ndrop + nmerge])),) + a.shape[ndrop + nmerge:])
+
+
+def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi, padding,
+                              fill_value, post_metric_fn):
+    """A built-in operator on a numpy field of a grid with face connections through the host slab pipeline
+    (``xg_stencil2_host_connected``), or None when the field does not stream (``_host_stream_route``)."""
+    from . import ops
+    from .padding import (_axis_dim, _get_all_connection_axes, _unpack_vector, connected_edge_mode,
+                          connected_halo_program)
+
+    da, isvector, vectoraxis, partner = _unpack_vector(grid, raw_arg, other_component)
+    if not _is_host_float(da) or grid._device_for(da).type != "cuda":
+        return None
+    dims, shape = tuple(da.dims), [int(v) for v in da.shape]
+    facedim = grid._facedim
+    core = [in_dim, facedim]
+    for axname in _get_all_connection_axes(grid._face_connections, facedim):
+        core += [d for d in grid.axes[axname].coords.values() if d in dims]
+    mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, shape[dims.index(facedim)])
+    axis_num = dims.index(in_dim)
+    out_dims = tuple(out_dim if d == in_dim else d for d in dims)
+    out_shape = list(shape)
+    out_shape[axis_num] = shape[axis_num] + lo + hi - 1
+    post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
+    post_h = None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype)
+    first = min(dims.index(d) for d in core)
+    partner_ok = not isvector or (
+        not partner.is_device and isinstance(partner.data, np.ndarray) and len(partner.dims) == len(dims)
+        and tuple(partner.dims[:first]) == dims[:first] and tuple(partner.shape[:first]) == tuple(shape[:first]))
+    route = _host_stream_route("connected", dims, shape, core, lo, hi, partner_ok=partner_ok,
+                               operand_shapes=[post_h.shape] if post_h is not None else [])
+    if route is None:
+        return None
+    _, ndrop, nmerge = route
+    cut = lambda a: _merge_leading(a, ndrop, nmerge)  # noqa: E731
+    lead = ndrop + nmerge
+    m_dims = dims[ndrop:ndrop + 1] + dims[lead:]  # the merged batch dim keeps the name of its first dim
+    x = cut(da.data)
+    q = partner_layout = None
+    if isvector:
+        q = cut(partner.data)
+        partner_layout = (tuple(partner.dims[ndrop:ndrop + 1] + partner.dims[lead:]), tuple(q.shape))
+    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, list(x.shape), mode, vectoraxis,
+                                     partner_layout)
+    out = ops.stencil2_host_connected(x, m_dims.index(in_dim), op, lo, hi, fv, program, partner=q,
+                                      post=None if post_h is None else cut(post_h),
+                                      device=grid._device_for(da).index)
+    return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
 
 
 class _ShapeProbe:

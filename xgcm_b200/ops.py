@@ -574,8 +574,22 @@ def stencil2_host(
     """Host-buffer twin of :func:`stencil2`: slabs stream H2D -> kernel -> D2H on three
     streams inside ``xg_stencil2_host``.  Page-locked buffers get the full PCIe rate."""
     lib = _capi.load()
+    x, shape, axis, out, pre_op, post_op, dev = _host_stencil_prep(x, axis, op, lo, hi, padding, pre, post, out,
+                                                                   device, "stencil2_host")
+    rc = lib.xg_stencil2_host(
+        _capi.OPS[op], _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim,
+        _capi.i64_array(shape), axis, lo, hi, _capi.BCS[padding], float(fill_value),
+        pre_op[1], pre_op[2], post_op[1], post_op[2], dev,
+    )
+    _capi.check(rc)
+    return out
+
+
+def _host_stencil_prep(x, axis, op, lo, hi, padding, pre, post, out, device, what):
+    """Checks and buffers shared by the host stencil twins: (contiguous x, shape, axis, out, pre operand,
+    post operand, device index)."""
     if not isinstance(x, np.ndarray):
-        raise TypeError("stencil2_host takes numpy arrays")
+        raise TypeError(f"{what} takes numpy arrays")
     if not torch.cuda.is_available():
         raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
     if op not in _capi.OPS:
@@ -594,13 +608,69 @@ def stencil2_host(
         out = pinned_empty(out_shape, x.dtype)
     elif list(out.shape) != out_shape or out.dtype != x.dtype or not out.flags.c_contiguous:
         raise ValueError("out has wrong shape/dtype/layout")
-    kp, pre_ptr, pre_st = _host_operand(pre, shape, x.dtype, "pre metric")
-    kq, post_ptr, post_st = _host_operand(post, out_shape, x.dtype, "post metric")
+    pre_op = _host_operand(pre, shape, x.dtype, "pre metric")
+    post_op = _host_operand(post, out_shape, x.dtype, "post metric")
     dev = torch.cuda.current_device() if device is None else int(device)
-    rc = lib.xg_stencil2_host(
+    return x, shape, axis, out, pre_op, post_op, dev
+
+
+def stencil2_host_fold(x: np.ndarray, axis: int, op: str, lo: int, hi: int, padding: Optional[str],
+                       fill_value: float, seam_axis: int, skip: int, mirror: int, period: int,
+                       negate: bool = False, pre: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None,
+                       out: Optional[np.ndarray] = None, device: Optional[int] = None) -> np.ndarray:
+    """:func:`stencil2_host` across a north fold along ``axis`` (``xg_stencil2_host_fold``): each slab's
+    halo_hi is its folded row (:func:`fold_rows` with ``seam_axis, skip, mirror, period, negate``, of
+    ``x * pre``), also halo_lo when the south edge ``padding`` is periodic.  Dim 0 is cut into slabs and must
+    be neither ``axis`` nor ``seam_axis``."""
+    lib = _capi.load()
+    x, shape, axis, out, pre_op, post_op, dev = _host_stencil_prep(x, axis, op, lo, hi, padding, pre, post, out,
+                                                                   device, "stencil2_host_fold")
+    rc = lib.xg_stencil2_host_fold(
         _capi.OPS[op], _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim,
         _capi.i64_array(shape), axis, lo, hi, _capi.BCS[padding], float(fill_value),
-        pre_ptr, pre_st, post_ptr, post_st, dev,
+        pre_op[1], pre_op[2], post_op[1], post_op[2], _norm_axis(seam_axis, x.ndim), int(skip), int(mirror),
+        int(period), 1 if negate else 0, dev,
+    )
+    _capi.check(rc)
+    return out
+
+
+_HALO_SOURCES = {"self": 0, "partner": 1, "fill": 2}
+
+
+def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int, fill_value: float,
+                            program: Sequence[tuple], partner: Optional[np.ndarray] = None,
+                            post: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
+                            device: Optional[int] = None) -> np.ndarray:
+    """:func:`stencil2_host` on a grid with face connections (``xg_stencil2_host_connected``): the halo
+    planes of each slab are written by ``program``, the strided copies of
+    ``padding.connected_halo_program`` — ``(side, dst offset, dst strides, source ("self", "partner" or
+    "fill"), src offset, src strides, shape, negate)`` for the whole field, clipped to each slab by the
+    library.  ``partner`` (the other vector component) streams beside ``x``; "fill" reads ``fill_value``."""
+    import ctypes as C
+
+    lib = _capi.load()
+    x, shape, axis, out, _, post_op, dev = _host_stencil_prep(x, axis, op, lo, hi, "fill" if (lo or hi) else None,
+                                                              None, post, out, device, "stencil2_host_connected")
+    p_shape = None
+    if partner is not None:
+        partner = np.ascontiguousarray(partner, dtype=x.dtype)
+        p_shape = list(partner.shape)
+        if len(p_shape) != x.ndim:
+            raise ValueError(f"partner component of shape {tuple(p_shape)} has not the rank of the field {tuple(shape)}")
+    n = len(program)
+    cndim = len(program[0][6]) if n else 1
+    if any(len(c[6]) != cndim or len(c[2]) != cndim or len(c[5]) != cndim for c in program):
+        raise ValueError("stencil2_host_connected: every copy must have the same rank")
+    i32 = lambda vals: (C.c_int * max(n, 1))(*vals)  # noqa: E731
+    flat = lambda k: _capi.i64_array([int(v) for c in program for v in c[k]] or [0])  # noqa: E731
+    rc = lib.xg_stencil2_host_connected(
+        _capi.OPS[op], _capi.dtype_code(x.dtype), x.ctypes.data,
+        None if partner is None else partner.ctypes.data, _capi.i64_array(p_shape), out.ctypes.data, x.ndim,
+        _capi.i64_array(shape), axis, lo, hi, float(fill_value), post_op[1], post_op[2], n, cndim,
+        i32([int(c[0]) for c in program]), i32([_HALO_SOURCES[c[3]] for c in program]),
+        _capi.i64_array([int(c[1]) for c in program] or [0]), _capi.i64_array([int(c[4]) for c in program] or [0]),
+        flat(6), flat(2), flat(5), i32([1 if c[7] else 0 for c in program]), dev,
     )
     _capi.check(rc)
     return out

@@ -434,6 +434,128 @@ def _unpack_vector(grid, da, other_component):
     return da, isvector, vectoraxis, da_partner
 
 
+def connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face_offset=0):
+    """``(mode, fill value)`` of the unconnected edges of ``ax_name`` on a grid with face connections, after
+    the same validation the simply connected path performs in ``ops.stencil2`` / ``_apply_fused_stencil``."""
+    face_links = grid._face_connections[grid._facedim]
+    paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
+    fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
+    ax_padding = paddings[ax_name]
+    # an unknown string must not silently become a periodic halo on the unconnected edges
+    if isinstance(ax_padding, Mapping):
+        raise NotImplementedError(
+            "fold / per-side padding mappings are not supported on grids with face connections"
+        )
+    if ax_padding not in (None, "periodic", "fill", "extend"):
+        if ax_padding == "extrapolate":
+            raise NotImplementedError(
+                "padding='extrapolate' (an opt-in extension without a reference counterpart) is not available "
+                "for operators on grids with face connections; use fill / extend / periodic"
+            )
+        raise ValueError(
+            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {ax_padding!r}"
+        )
+    for side, w in ((0, lo), (1, hi)):
+        if not w:
+            continue
+        unconnected = [face_offset + i for i in range(n_face)
+                       if face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side] is None]
+        if ax_padding is None and unconnected:
+            raise ValueError(
+                f"No boundary condition was specified for axis {ax_name!r}, "
+                f"but the requested operation needs to pad the {'right' if side else 'left'} "
+                f"edge of face(s) {unconnected}, which have no face "
+                f"connection there. Set a boundary condition, e.g. "
+                f"``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
+                f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
+                f"grid method."
+            )
+    fv = fills[ax_name] if fills[ax_name] is not None else 0.0
+    return (ax_padding if ax_padding is not None else "fill"), float(fv)
+
+
+def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout, face_offset=0,
+                        remote_edges=None):
+    """The strided copies that write the neighbour rims of every connected edge into the one-cell halo
+    planes of a field with ``dims`` / ``shape`` along ``ax_name``: a list of ``(side, dst offset, dst strides,
+    source ("self" or "partner"), src offset, src strides, shape, negate)``, offsets and strides in elements
+    of the contiguous plane (``shape`` with extent 1 along the axis) and source arrays.  ``partner_layout``:
+    ``(dims, shape)`` of the other vector component, or None for a scalar.
+
+    The index maps depend only on the topology and the array layout, not on the values: they are derived
+    once per (axis, widths, layout) and kept on the grid.  ``face_offset`` / ``remote_edges`` as in
+    :func:`connected_halo_planes` (such plans are not cached)."""
+    facedim = grid._facedim
+    face_links = grid._face_connections[facedim]
+    isvector = partner_layout is not None
+    cache = grid.__dict__.setdefault("_halo_plan_cache", {})
+    key = (ax_name, lo, hi, tuple(dims), tuple(shape), vectoraxis, partner_layout)
+    plan = cache.get(key) if remote_edges is None else None
+    if plan is not None:
+        return plan
+    sources = {"self": ("self", tuple(dims), list(shape), _contiguous_strides(shape))}
+    if isvector:
+        p_dims, p_shape = partner_layout
+        sources["partner"] = ("partner", tuple(p_dims), list(p_shape), _contiguous_strides(p_shape))
+    t = list(dims).index(_axis_dim(grid, dims, ax_name))
+    n_face = shape[list(dims).index(facedim)]
+    p_shape = list(shape)
+    p_shape[t] = 1
+    plan = []
+    for side, w in ((0, lo), (1, hi)):
+        if not w:
+            continue
+        for i in range(n_face):
+            connection = face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side]
+            if not connection:
+                continue
+            src_local = connection[0] - face_offset
+            if remote_edges is not None and not 0 <= src_local < n_face:
+                remote_edges.append((side, i, connection))
+                continue
+            _copy_connected_edge(grid, facedim, side, tuple(dims), p_shape, i, ax_name, 0, 1, 0,
+                                 (src_local,) + tuple(connection[1:]), bool(side), sources, isvector,
+                                 vectoraxis, plan)
+    if remote_edges is None:
+        cache[key] = plan
+    return plan
+
+
+def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=None, partner_layout=None):
+    """Every strided copy that builds the one-cell halo planes of a field with ``dims`` / ``shape`` along
+    ``ax_name``, for the host slab pipeline (``xg_stencil2_host_connected``), which replays the list on each
+    slab: the neighbour rims of :func:`_connected_edge_plan` plus, on each face without a connection on a
+    padded side, the basic boundary value (``mode``: fill from the constant, source ``"fill"``; extend: the
+    nearest row; periodic: the row at the other end).  Each face's plane is written by exactly one copy."""
+    facedim = grid._facedim
+    face_links = grid._face_connections[facedim]
+    dims = tuple(dims)
+    t = dims.index(_axis_dim(grid, dims, ax_name))
+    f = dims.index(facedim)
+    n = shape[t]
+    strides = _contiguous_strides(shape)
+    p_shape = list(shape)
+    p_shape[t] = 1
+    p_strides = _contiguous_strides(p_shape)
+    loop = [d for d in range(len(dims)) if d != f]
+    program = list(_connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout))
+    for side, w in ((0, lo), (1, hi)):
+        if not w:
+            continue
+        for i in range(shape[f]):
+            if face_links.get(i, {}).get(ax_name, (None, None))[side] is not None:
+                continue
+            c_shape = [p_shape[d] for d in loop]
+            dst = (side, i * p_strides[f], [p_strides[d] for d in loop])
+            if mode == "fill":
+                program.append(dst + ("fill", 0, [0] * len(loop), c_shape, False))
+            else:
+                row = ((n - 1) if side else 0) if mode == "extend" else (0 if side else (n - 1))
+                program.append(dst + ("self", i * strides[f] + row * strides[t], [strides[d] for d in loop],
+                                      c_shape, False))
+    return program
+
+
 def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_component=None,
                           face_offset=0, remote_edges=None):
     """The one-cell halo planes of ``da`` along ``ax_name`` on a grid with face connections, for
@@ -456,7 +578,6 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
     from .device import as_device_tensor
 
     facedim = grid._facedim
-    face_links = grid._face_connections[facedim]
     da, isvector, vectoraxis, da_partner = _unpack_vector(grid, da, other_component)
     x, was_host = as_device_tensor(da.data, grid._device_for(da))
     dims = tuple(da.dims)
@@ -473,46 +594,15 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
     t = dims.index(target_dim)
     n = shape[t]
     n_face = shape[dims.index(facedim)]
-    paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
-    fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
-    ax_padding = paddings[ax_name]
-    # the same validation the simply connected path performs in ops.stencil2 / _apply_fused_stencil: an
-    # unknown string must not silently become a periodic halo on the unconnected edges
-    if isinstance(ax_padding, Mapping):
-        raise NotImplementedError(
-            "fold / per-side padding mappings are not supported on grids with face connections"
-        )
-    if ax_padding not in (None, "periodic", "fill", "extend"):
-        if ax_padding == "extrapolate":
-            raise NotImplementedError(
-                "padding='extrapolate' (an opt-in extension without a reference counterpart) is not available "
-                "for operators on grids with face connections; use fill / extend / periodic"
-            )
-        raise ValueError(
-            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {ax_padding!r}"
-        )
-    planes, batch = [], []
+    mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face_offset)
+    planes = []
     for side, w in ((0, lo), (1, hi)):
         if not w:
             planes.append(None)
             continue
-        unconnected = [face_offset + i for i in range(n_face)
-                       if face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side] is None]
-        if ax_padding is None and unconnected:
-            raise ValueError(
-                f"No boundary condition was specified for axis {ax_name!r}, "
-                f"but the requested operation needs to pad the {'right' if side else 'left'} "
-                f"edge of face(s) {unconnected}, which have no face "
-                f"connection there. Set a boundary condition, e.g. "
-                f"``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                f"grid method."
-            )
         p_shape = list(shape)
         p_shape[t] = 1
-        mode = ax_padding if ax_padding is not None else "fill"
         if mode == "fill":
-            fv = fills[ax_name] if fills[ax_name] is not None else 0.0
             plane = torch.full(p_shape, float(fv), dtype=x.dtype, device=x.device)
         else:  # extend: nearest cell; periodic: the cell at the other end
             plane = torch.empty(p_shape, dtype=x.dtype, device=x.device)
@@ -524,36 +614,9 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
             ops.strided_copy(plane, 0, _contiguous_strides(p_shape), x, row * strides[t], strides, p_shape)
         planes.append(plane)
 
-    # The index maps of the connected edges depend only on the topology and the array layout, not
-    # on the values: derive them once per (axis, widths, layout) and keep them on the grid.
-    cache = grid.__dict__.setdefault("_halo_plan_cache", {})
-    key = (ax_name, lo, hi, dims, tuple(shape), vectoraxis,
-           None if not isvector else (sources["partner"][1], tuple(sources["partner"][2])))
-    plan = cache.get(key) if remote_edges is None else None
-    if plan is None:
-        plan = []
-        p_shape = list(shape)
-        p_shape[t] = 1
-        for side, w in ((0, lo), (1, hi)):
-            if not w:
-                continue
-            for i in range(n_face):
-                connection = face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side]
-                if not connection:
-                    continue
-                src_local = connection[0] - face_offset
-                if remote_edges is not None and not 0 <= src_local < n_face:
-                    remote_edges.append((side, i, connection))
-                    continue
-                one = []
-                _copy_connected_edge(grid, facedim, planes[side], dims, p_shape, i, ax_name, 0, 1, 0,
-                                     (src_local,) + tuple(connection[1:]), bool(side), sources, isvector,
-                                     vectoraxis, one)
-                for _, doff, dstr, src, soff, sstr, shp, neg in one:
-                    src_key = "partner" if (isvector and src is sources["partner"][0]) else "self"
-                    plan.append((side, doff, dstr, src_key, soff, sstr, shp, neg))
-        if remote_edges is None:
-            cache[key] = plan
+    partner_layout = None if not isvector else (sources["partner"][1], tuple(sources["partner"][2]))
+    plan = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout,
+                                face_offset, remote_edges)
     batch = [(planes[side], doff, dstr, sources[src_key][0], soff, sstr, shp, neg)
              for side, doff, dstr, src_key, soff, sstr, shp, neg in plan]
     ops.strided_copy_batch(batch)  # both planes, every connected face: one launch
