@@ -175,21 +175,24 @@ def test_wreduce_strided_exact(dtype):
                 np.testing.assert_array_equal(got, want)
 
 
-@pytest.mark.parametrize("dtype,rtol", [(np.float32, 1e-6), (np.float64, 1e-12)])
-def test_wreduce_rows_and_mean(dtype, rtol):
+@pytest.mark.parametrize("dtype", [np.float32, np.float64])
+def test_wreduce_rows_and_mean(dtype):
+    """Row reductions (fp64 accumulation, one rounding) against the exact sum; strided means bit-exact."""
+    from test_kernel_instances_gpu import _fsum_bound_check
     from xgcm_b200 import ops
 
     shape = (7, 9, 1000)
     a = _field(shape, dtype, seed=18, nan_frac=0.02)
     w = (0.5 + np.random.default_rng(19).random((1, 1, 1000))).astype(dtype)
-    want = oracle.wreduce(a, w, 2, "sum", True)
     got = ops.wreduce(_t(a), 2, _t(w), "sum", True).cpu().numpy()
-    np.testing.assert_allclose(got, want, rtol=rtol)
+    _fsum_bound_check(got, a, w, 2, "sum", True, "rows sum")
     for axis in range(3):
         for wt in (None, (0.5 + np.random.default_rng(20).random(shape)).astype(dtype)):
-            want = oracle.wreduce(a, wt, axis, "mean", True)
             got = ops.wreduce(_t(a), axis, _t(wt), "mean", True).cpu().numpy()
-            np.testing.assert_allclose(got, want, rtol=rtol * 4, equal_nan=True)
+            if axis == 2:
+                _fsum_bound_check(got, a, wt, 2, "mean", True, "rows mean")
+            else:
+                np.testing.assert_array_equal(got, oracle.wreduce(a, wt, axis, "mean", True))
     allnan = np.full((4, 5), np.nan, dtype=dtype)
     got = ops.wreduce(_t(allnan), 0, None, "mean", True).cpu().numpy()
     assert np.isnan(got).all()  # xarray weighted mean: 0/0 -> NaN
@@ -198,16 +201,16 @@ def test_wreduce_rows_and_mean(dtype, rtol):
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_wreduce_rows_vector_and_scalar_loads(dtype):
     """The innermost-axis reduction reads 16-byte vectors when the rows allow it, else single elements."""
+    from test_kernel_instances_gpu import _fsum_bound_check
     from xgcm_b200 import _capi, ops
 
-    rtol = 1e-6 if dtype == np.float32 else 1e-12
     for n, side in ((1000, "vec"), (999, "scalar")):
         a = _field((7, 9, n), dtype, seed=21, nan_frac=0.02)
         w = (0.5 + np.random.default_rng(22).random((1, 1, n))).astype(dtype)
         for mode in ("sum", "mean"):
             got = ops.wreduce(_t(a), 2, _t(w), mode, True).cpu().numpy()
             assert _capi.last_launch() == f"xg_wreduce(rows, {side})"
-            np.testing.assert_allclose(got, oracle.wreduce(a, w, 2, mode, True), rtol=rtol * 4, equal_nan=True)
+            _fsum_bound_check(got, a, w, 2, mode, True, f"n={n} {mode}")
 
 
 # ----------------------------------------------------------------------------- strided scan / reduce at the 16-byte switch
@@ -359,10 +362,11 @@ def test_vinterp_log(dtype):
 
 @pytest.mark.parametrize("dtype", [np.float32, np.float64])
 def test_vinterp_shared_slope_division_is_correctly_rounded(dtype):
-    """The shared-theta kernel forms slope = dy/dx from a precomputed reciprocal plus FMA corrections;
-    it must round exactly like the reference's fp64 division: many columns, wide dynamic range,
-    zeros, NaNs, non power-of-two spacings."""
-    from xgcm_b200 import ops
+    """The shared-theta kernels form slope = dy/dx from a precomputed reciprocal plus FMA corrections;
+    they must round exactly like the reference's fp64 division: many columns, wide dynamic range,
+    zeros, NaNs, non power-of-two spacings.  An aligned phi takes the TMA kernel; a phi one element
+    past a 16-byte boundary (a time slice of a larger field) the fallback k_vinterp_shared."""
+    from xgcm_b200 import _capi, ops
 
     rng = np.random.default_rng(77)
     ncol, n = 200_000, 5
@@ -373,8 +377,12 @@ def test_vinterp_shared_slope_division_is_correctly_rounded(dtype):
     theta = np.array([0.1, 0.7, 1.9, 3.0000001, 7.3], dtype=dtype).reshape(n, 1)
     target = np.array([0.05, 0.1, 0.33, 0.7000001, 1.0, 2.5, 3.0, 3.5, 7.0, 7.3, 9.0], dtype=dtype)
     want = oracle.vinterp_linear(phi, np.broadcast_to(theta, phi.shape), target, 0, True)
-    got = ops.vinterp_linear(_t(phi), _t(theta), _t(target), 0, True).cpu().numpy()
-    np.testing.assert_array_equal(got, want)
+    shifted = torch.empty(phi.size + 1, dtype=_t(phi).dtype, device=DEV)[1:].view(phi.shape)
+    shifted.copy_(torch.from_numpy(phi))
+    for field, label in ((_t(phi), "xg_vinterp_linear(shared, tma)"), (shifted, "xg_vinterp_linear(shared)")):
+        got = ops.vinterp_linear(field, _t(theta), _t(target), 0, True).cpu().numpy()
+        assert _capi.last_launch() == label
+        np.testing.assert_array_equal(got, want)
 
 
 def test_vinterp_mixed_dtypes_promote_like_numba():

@@ -275,15 +275,11 @@ int launch_op(int op, const MultiArgs<T>& a, int64_t nblocks, int threads, cudaS
 template <typename T, int VEC, int K, int LAST>
 int launch_march(int march, const MultiArgs<T>& a, int64_t nblocks, int threads, cudaStream_t st) {
   const int op = a.ax[0].op;  // the fused kernel applies one operator along all axes
-  // MARCH is a row-axis op, so MARCH != LAST
-  if (march == 0) {
-    if constexpr (LAST != 0) return launch_op<T, VEC, K, LAST, 0>(op, a, nblocks, threads, st);
-  } else if (march == 1) {
-    if constexpr (LAST != 1) return launch_op<T, VEC, K, LAST, 1>(op, a, nblocks, threads, st);
-  } else if (march == 2) {
-    if constexpr (K == 3 && LAST != 2) return launch_op<T, VEC, K, LAST, 2>(op, a, nblocks, threads, st);
-  }
-  return xg_fail(XG_EINVAL, "xg_stencil_multi: bad march axis");
+  // multi_typed marches along the highest application index other than LAST; only that MARCH is
+  // instantiated for each (K, LAST)
+  constexpr int MARCH = LAST == K - 1 ? K - 2 : K - 1;
+  if (march != MARCH) return xg_fail(XG_EINVAL, "xg_stencil_multi: bad march axis");
+  return launch_op<T, VEC, K, LAST, MARCH>(op, a, nblocks, threads, st);
 }
 
 template <typename T, int VEC, int K>

@@ -89,7 +89,9 @@ __global__ void __launch_bounds__(kThreads) k_reduce_strided(const ReduceArgs<T>
   xg_st_stream<T, VEC>(a.out + o * a.inner + i, r);
 }
 
-// one warp per row (innermost axis); fp64 accumulation; 16-byte loads when the rows allow it
+// one warp per row (innermost axis); fp64 accumulation; 16-byte loads when the rows allow it.  Either way a lane
+// sums the same cells in the same order (W consecutive cells every 32 W), so a row gives the same bits whether it
+// is aligned or not: x[t] of a (T, Z, Y, X) field and x[t].clone() agree.
 template <typename T, bool HASW, int VEC>
 __global__ void __launch_bounds__(kThreads) k_reduce_rows(const ReduceArgs<T> a) {
   const int64_t r = (int64_t)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5);
@@ -101,10 +103,19 @@ __global__ void __launch_bounds__(kThreads) k_reduce_rows(const ReduceArgs<T> a)
   if (HASW) w_base = xg_groups_offset(a.w.outer, r);
   const bool mean = a.mode != XG_REDUCE_SUM;
   double num = 0.0, den = 0.0;
-  for (int64_t x = (int64_t)lane * VEC; x < a.n; x += 32 * VEC) {
-    XgPack<T, VEC> v = xg_ld_stream<T, VEC>(row + x);
+  constexpr int W = XgVecWidth<T>::value;
+  for (int64_t x = (int64_t)lane * W; x < a.n; x += 32 * W) {
+    XgPack<T, W> v;
+    if constexpr (VEC == W) {
+      v = xg_ld_stream<T, W>(row + x);
+    } else {
 #pragma unroll
-    for (int q = 0; q < VEC; ++q) {
+      for (int q = 0; q < W; ++q)
+        if (x + q < a.n) v.v[q] = xg_ld_stream<T, 1>(row + x + q).v[0];
+    }
+#pragma unroll
+    for (int q = 0; q < W; ++q) {
+      if (VEC != W && x + q >= a.n) break;
       const T w = HASW ? __ldg(wp + w_base + (x + q) * a.w.axis_stride) : T(1);
       if (!mean) {
         T p = HASW ? v.v[q] * w : v.v[q];
