@@ -154,6 +154,20 @@ XG_API int xg_stencil_pair(int dtype, const void* a, const void* b, void* out, i
                     const int64_t* post_strides, void* stream);
 
 /*
+ * xg_stencil_pair with optional halo planes for the term along axis_b (e.g. the folded north row of a
+ * tripolar grid).  halo_lo_b / halo_hi_b: contiguous device planes of the common shape with extent 1
+ * along axis_b, already weighted (b * pre_b at their source cell, as the halo planes of xg_stencil2);
+ * each replaces bc_b on its side.  NULL planes: exactly xg_stencil_pair.
+ */
+XG_API int xg_stencil_pair_halo(int dtype, const void* a, const void* b, void* out, int ndim,
+                                const int64_t* shape, int op_a, int lo_a, int hi_a, int bc_a, double fill_a,
+                                const void* pre_a, const int64_t* pre_a_strides, int axis_b, int op_b,
+                                int lo_b, int hi_b, int bc_b, double fill_b, const void* pre_b,
+                                const int64_t* pre_b_strides, int subtract, const void* post,
+                                const int64_t* post_strides, const void* halo_lo_b, const void* halo_hi_b,
+                                void* stream);
+
+/*
  * Cumulative sum along one axis with xgcm's position-shift bookkeeping:
  * c = cumsum(in * pre) (from the high end when reverse), then trim, then pad
  * (pad_lo, pad_hi in {0,1}) with `bc` applied to the cumsum'd data, then / post.
@@ -341,7 +355,33 @@ XG_API int xg_stencil2_host_connected(int op, int dtype, const void* in, const v
                                       const int64_t* shapes, const int64_t* dst_strides,
                                       const int64_t* src_strides, const int* negate, int device);
 
-/* Device bytes the workspace of xg_stencil2_host and its _fold / _connected variants holds on `device`
+/*
+ * Host-buffer twins of xg_stencil_pair: same semantics, HOST pointers, `device` instead of a stream;
+ * synchronous.  The slab pipeline of xg_stencil2_host: `a` is cut into slabs along dim 0, `b` streams
+ * beside it slab by slab, pre_a / pre_b / post are uploaded whole.  Dim 0 must be a batch dim: not axis_b
+ * (nor the innermost dim, nor the seam dim of _fold) (XG_EINVAL).  Every argument is checked before any
+ * CUDA call.
+ *
+ * _fold: the term along axis_b crosses a north fold (hi_b must be 1).  Per slab, one xg_fold_rows launch
+ * of b * pre_b (width 1; seam_axis, skip, mirror, period, negate as there) writes halo_hi_b of
+ * xg_stencil_pair_halo; with lo_b = 1 and bc_b = XG_BC_PERIODIC it is halo_lo_b too.  XG_ENOTIMPL where
+ * xg_fold_rows would return it.
+ */
+XG_API int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim,
+                                const int64_t* shape, int op_a, int lo_a, int hi_a, int bc_a, double fill_a,
+                                const void* pre_a, const int64_t* pre_a_strides, int axis_b, int op_b,
+                                int lo_b, int hi_b, int bc_b, double fill_b, const void* pre_b,
+                                const int64_t* pre_b_strides, int subtract, const void* post,
+                                const int64_t* post_strides, int device);
+XG_API int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, void* out, int ndim,
+                                     const int64_t* shape, int op_a, int lo_a, int hi_a, int bc_a,
+                                     double fill_a, const void* pre_a, const int64_t* pre_a_strides,
+                                     int axis_b, int op_b, int lo_b, int hi_b, int bc_b, double fill_b,
+                                     const void* pre_b, const int64_t* pre_b_strides, int subtract,
+                                     const void* post, const int64_t* post_strides, int seam_axis, int skip,
+                                     int64_t mirror, int64_t period, int negate, int device);
+
+/* Device bytes the workspace of xg_stencil2_host, xg_stencil_pair_host and their variants holds on `device`
  * (slot buffers, metrics, halo planes); 0 before the first call or after xg_host_workspace_release. */
 XG_API int xg_host_workspace_bytes(int device, int64_t* bytes);
 

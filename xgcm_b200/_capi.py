@@ -123,6 +123,22 @@ SIGNATURES = {
         [C.c_int, _vp, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p,
          C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p, C.c_int, _vp, _i64p, _vp],
     ),
+    "xg_stencil_pair_halo": (
+        C.c_int,
+        [C.c_int, _vp, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p,
+         C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p, C.c_int, _vp, _i64p, _vp, _vp, _vp],
+    ),
+    "xg_stencil_pair_host": (
+        C.c_int,
+        [C.c_int, _vp, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p,
+         C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p, C.c_int, _vp, _i64p, C.c_int],
+    ),
+    "xg_stencil_pair_host_fold": (
+        C.c_int,
+        [C.c_int, _vp, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p,
+         C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p, C.c_int, _vp, _i64p,
+         C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int, C.c_int],
+    ),
     "xg_nccl_load": (C.c_int, [C.c_char_p]),
     "xg_comm_unique_id": (C.c_int, [_vp]),
     "xg_comm_init": (C.c_int, [_vp, C.c_int, C.c_int, _vpp]),

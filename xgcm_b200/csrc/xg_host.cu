@@ -15,6 +15,10 @@
 // xg_strided_copy_batch) just before its xg_stencil2 launch.  Dim 0 is then a batch dim, so the planes
 // of one slab depend on that slab (and the partner component's slab) alone.
 //
+// xg_stencil_pair_host / xg_stencil_pair_host_fold run the two-field composite on the same loop: field a
+// is the slab input, field b streams through the partner slots, and each slab is one xg_stencil_pair_halo
+// launch (after the xg_fold_rows launch of b's folded row, for the fold).
+//
 // Workspace (device slabs + events + streams) is cached per device and reused;
 // xg_host_workspace_release() frees it.
 #include <stdlib.h>
@@ -31,12 +35,12 @@ constexpr int kSlots = 3;
 struct Workspace {
   int device = -1;
   std::mutex mu;  // one host call at a time per device; different devices run concurrently
-  size_t slab_in_bytes = 0, slab_out_bytes = 0, metric_bytes[2] = {0, 0}, halo_bytes = 0;
+  size_t slab_in_bytes = 0, slab_out_bytes = 0, metric_bytes[3] = {0, 0, 0}, halo_bytes = 0;
   size_t partner_bytes = 0, const_bytes = 0;
   void* d_in[kSlots] = {nullptr, nullptr, nullptr};
   void* d_out[kSlots] = {nullptr, nullptr, nullptr};
-  void* d_partner[kSlots] = {nullptr, nullptr, nullptr};  // second vector component (face connections)
-  void* d_metric[2] = {nullptr, nullptr};
+  void* d_partner[kSlots] = {nullptr, nullptr, nullptr};  // second vector component, or field b of a pair
+  void* d_metric[3] = {nullptr, nullptr, nullptr};       // pre, post, and pre_a of a pair
   void* d_halo[2] = {nullptr, nullptr};  // wrap planes along dim 0, or the per-slab lo / hi halo planes
   void* d_const = nullptr;               // the fill constant the unconnected face edges copy from
   cudaStream_t s_h2d = nullptr, s_k = nullptr, s_d2h = nullptr;
@@ -114,10 +118,10 @@ extern "C" int xg_host_workspace_release(void) {
         cudaEventDestroy(w->e_down[i]);
       }
     }
-    for (int i = 0; i < 2; ++i) {
+    for (int i = 0; i < 3; ++i)
       if (w->d_metric[i]) cudaFree(w->d_metric[i]);
+    for (int i = 0; i < 2; ++i)
       if (w->d_halo[i]) cudaFree(w->d_halo[i]);
-    }
     if (w->d_const) cudaFree(w->d_const);
     if (w->s_h2d) cudaStreamDestroy(w->s_h2d);
     if (w->s_k) cudaStreamDestroy(w->s_k);
@@ -129,6 +133,17 @@ extern "C" int xg_host_workspace_release(void) {
 }
 
 namespace {
+
+// The x term and the second field of xg_stencil_pair_host.  Its Call describes the term along `axis`
+// (op_b, lo_b, hi_b, bc_b, fill_b, pre_b) and `post`, and its `in` is field a, the slab input.
+struct PairTerm {
+  const void* b;
+  int op_a, lo_a, hi_a, bc_a;
+  double fill_a;
+  const void* pre_a;
+  const int64_t* pre_a_strides;
+  int subtract;
+};
 
 // The stencil call the slab loop runs, slab by slab.
 struct Call {
@@ -144,6 +159,7 @@ struct Call {
   const void* post;
   const int64_t* post_strides;
   int device;
+  const PairTerm* pair = nullptr;  // xg_stencil_pair_halo instead of xg_stencil2
 };
 
 enum { kHaloNone = 0, kHaloFold = 1, kHaloCopies = 2 };
@@ -196,6 +212,48 @@ int validate_halo_call(const char* who, const Call& c) {
   return XG_OK;
 }
 
+// The fold parameters of the _fold entry points (the checks xg_fold_rows makes, before any CUDA call).
+int validate_fold(const char* who, const Call& c, int seam_axis, int skip, int64_t mirror, int64_t period) {
+  const std::string w(who);
+  if (seam_axis < 0 || seam_axis >= c.ndim) return xg_fail(XG_EINVAL, w + ": seam axis out of range");
+  if (seam_axis == 0) return xg_fail(XG_EINVAL, w + ": dim 0 is cut into slabs and must not be the seam dim");
+  if (seam_axis == c.axis) return xg_fail(XG_EINVAL, w + ": the fold and seam axes must differ");
+  if (c.hi != 1) return xg_fail(XG_EINVAL, w + ": the fold is the upper halo: hi must be 1");
+  if (skip < 0 || skip > 1) return xg_fail(XG_EINVAL, w + ": skip must be 0 or 1");
+  if (c.shape[c.axis] - skip < 1)
+    return xg_fail(XG_EINVAL, w + ": halo width exceeds the interior rows of the fold axis");
+  if (period < 1) return xg_fail(XG_EINVAL, w + ": period must be positive");
+  for (int64_t k = 0; k < c.shape[seam_axis]; ++k) {
+    int64_t src = (mirror - k) % period;
+    if (src < 0) src += period;
+    if (src >= c.shape[seam_axis])
+      return xg_fail(XG_ENOTIMPL, w + ": seam position incompatible with the pivot: the mirror "
+                                      "partner of a seam index lies outside the seam dim");
+  }
+  return XG_OK;
+}
+
+// The checks xg_stencil_pair makes, plus those of the slab loop (dim 0 a batch dim), before any CUDA call.
+int validate_pair_call(const char* who, const Call& c) {
+  const std::string w(who);
+  const PairTerm& t = *c.pair;
+  if (!t.b) return xg_fail(XG_EINVAL, w + ": null pointer");
+  int rc = validate_halo_call(who, c);
+  if (rc) return rc;
+  if (c.axis >= c.ndim - 1) return xg_fail(XG_EINVAL, w + ": axis_b must be a dimension other than the innermost one");
+  if (t.lo_a < 0 || t.hi_a < 0 || t.lo_a + t.hi_a != 1 || c.lo + c.hi != 1)
+    return xg_fail(XG_ENOTIMPL, w + ": both stencils must be length preserving (lo + hi == 1)");
+  for (int bc : {t.bc_a, c.bc})
+    if (bc < XG_BC_PERIODIC || bc > XG_BC_EXTEND)
+      return xg_fail(XG_EINVAL, w + ": boundary must be periodic, fill or extend");
+  for (int op : {t.op_a, c.op})
+    if (op < XG_OP_DIFF || op > XG_OP_MAX) return xg_fail(XG_EINVAL, w + ": unknown op");
+  if (t.pre_a && !t.pre_a_strides) return xg_fail(XG_EINVAL, w + ": metric strides missing");
+  if (t.subtract < 0 || t.subtract > 2) return xg_fail(XG_EINVAL, w + ": subtract must be 0, 1 or 2");
+  if (c.in == c.out || t.b == c.out) return xg_fail(XG_EINVAL, w + ": in-place operation is not supported");
+  return XG_OK;
+}
+
 // Per-slab face-connection copies: rebase the whole-field copy list onto the slab buffers, `rows` high.
 int halo_copies(const HaloStage& h, int dtype, size_t es, void* const planes[2], const void* field,
                 const void* partner, const void* fill, int64_t rows, std::vector<void*>& dptr,
@@ -243,6 +301,8 @@ int run_slabs(const Call& c, const HaloStage& h) {
   }
   const int64_t n0_out = out_shape[0];
   if (n0_out <= 0 || row_out == 0 || row_in == 0) return XG_OK;
+  const void* partner = c.pair ? c.pair->b : h.partner;
+  const int64_t partner_row = c.pair ? row_in : h.partner_row;
   const bool ax0 = axis == 0;
 
   // slab height along dim 0: ~128 MiB of input per slab, at least 4 slabs if possible
@@ -271,8 +331,8 @@ int run_slabs(const Call& c, const HaloStage& h) {
     if (rc) return rc;
     rc = ensure(&w->d_out[i], &have_out, (size_t)(rows * row_out) * es);
     if (rc) return rc;
-    if (h.partner) {
-      rc = ensure(&w->d_partner[i], &have_p, (size_t)(rows * h.partner_row) * es);
+    if (partner) {
+      rc = ensure(&w->d_partner[i], &have_p, (size_t)(rows * partner_row) * es);
       if (rc) return rc;
     }
     if (i == kSlots - 1) {
@@ -283,10 +343,10 @@ int run_slabs(const Call& c, const HaloStage& h) {
   }
   // (all three slots share one recorded capacity: grow them together)
   // metrics: uploaded whole, once
-  const void* hm[2] = {c.pre, c.post};
-  const int64_t* ms[2] = {c.pre_strides, c.post_strides};
-  const int64_t* mshape[2] = {shape, out_shape};
-  for (int k = 0; k < 2; ++k) {
+  const void* hm[3] = {c.pre, c.post, c.pair ? c.pair->pre_a : nullptr};
+  const int64_t* ms[3] = {c.pre_strides, c.post_strides, c.pair ? c.pair->pre_a_strides : nullptr};
+  const int64_t* mshape[3] = {shape, out_shape, shape};
+  for (int k = 0; k < 3; ++k) {
     if (!hm[k]) continue;
     const size_t span = operand_span(ms[k], mshape[k], ndim, es);
     rc = ensure(&w->d_metric[k], &w->metric_bytes[k], span);
@@ -378,10 +438,9 @@ int run_slabs(const Call& c, const HaloStage& h) {
       XG_CUDA(cudaMemcpyAsync(w->d_in[slot], hin + (size_t)i0 * row_in * es,
                               (size_t)(i1 - i0) * row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
     }
-    if (h.partner)
-      XG_CUDA(cudaMemcpyAsync(w->d_partner[slot],
-                              static_cast<const char*>(h.partner) + (size_t)(i0 * h.partner_row) * es,
-                              (size_t)((i1 - i0) * h.partner_row) * es, cudaMemcpyHostToDevice, w->s_h2d));
+    if (partner)
+      XG_CUDA(cudaMemcpyAsync(w->d_partner[slot], static_cast<const char*>(partner) + (size_t)(i0 * partner_row) * es,
+                              (size_t)((i1 - i0) * partner_row) * es, cudaMemcpyHostToDevice, w->s_h2d));
     prev_last_row = i1 - 1;
     prev_last_ptr = (const char*)w->d_in[slot] + (size_t)(i1 - 1 - i0) * row_in * es;
     XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
@@ -392,6 +451,8 @@ int run_slabs(const Call& c, const HaloStage& h) {
     const char* qm = (const char*)w->d_metric[1];
     if (c.pre) pm += (size_t)(i0 * c.pre_strides[0]) * es;
     if (c.post) qm += (size_t)(j0 * c.post_strides[0]) * es;
+    const char* am = (const char*)w->d_metric[2];
+    if (c.pair && c.pair->pre_a) am += (size_t)(i0 * c.pair->pre_a_strides[0]) * es;
     const void* hl = nullptr;
     const void* hh = nullptr;
     if (ax0 && wrap_planes) {
@@ -399,8 +460,9 @@ int run_slabs(const Call& c, const HaloStage& h) {
       if (slab_hi) hh = w->d_halo[1];
     }
     if (h.kind == kHaloFold) {
-      rc = xg_fold_rows(c.dtype, w->d_in[slot], w->d_halo[1], ndim, slab_shape, axis, h.seam_axis, 1, 0, 1,
-                        h.skip, h.mirror, h.period, h.negate, c.pre ? pm : nullptr, c.pre_strides, w->s_k);
+      rc = xg_fold_rows(c.dtype, c.pair ? w->d_partner[slot] : w->d_in[slot], w->d_halo[1], ndim, slab_shape, axis,
+                        h.seam_axis, 1, 0, 1, h.skip, h.mirror, h.period, h.negate, c.pre ? pm : nullptr,
+                        c.pre_strides, w->s_k);
       hh = w->d_halo[1];
       if (lo && bc == XG_BC_PERIODIC) hl = hh;  // a periodic south edge wraps the row above the top
     } else if (h.kind == kHaloCopies) {
@@ -409,10 +471,17 @@ int run_slabs(const Call& c, const HaloStage& h) {
       if (lo) hl = w->d_halo[0];
       if (hi) hh = w->d_halo[1];
     }
-    if (rc == XG_OK)
+    if (rc == XG_OK && c.pair) {
+      const PairTerm& t = *c.pair;
+      rc = xg_stencil_pair_halo(c.dtype, w->d_in[slot], w->d_partner[slot], w->d_out[slot], ndim, slab_shape, t.op_a,
+                                t.lo_a, t.hi_a, t.bc_a, t.fill_a, t.pre_a ? am : nullptr, t.pre_a_strides, axis, c.op,
+                                lo, hi, bc, c.fill_value, c.pre ? pm : nullptr, c.pre_strides, t.subtract,
+                                c.post ? qm : nullptr, c.post_strides, hl, hh, w->s_k);
+    } else if (rc == XG_OK) {
       rc = xg_stencil2(c.op, c.dtype, w->d_in[slot], w->d_out[slot], ndim, slab_shape, axis, slab_lo, slab_hi,
                        (slab_lo || slab_hi) ? bc : XG_BC_NONE, c.fill_value, c.pre ? pm : nullptr,
                        c.pre_strides, c.post ? qm : nullptr, c.post_strides, hl, hh, w->s_k);
+    }
     if (rc) {
       cudaDeviceSynchronize();
       return rc;
@@ -463,24 +532,8 @@ extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* ou
   const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, bc, fill_value,
                pre_metric, pre_strides, post_metric, post_strides, device};
   int rc = validate_halo_call(who, c);
+  if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
   if (rc) return rc;
-  if (seam_axis < 0 || seam_axis >= ndim) return xg_fail(XG_EINVAL, std::string(who) + ": seam axis out of range");
-  if (seam_axis == 0)
-    return xg_fail(XG_EINVAL, std::string(who) + ": dim 0 is cut into slabs and must not be the seam dim");
-  if (seam_axis == axis)
-    return xg_fail(XG_EINVAL, std::string(who) + ": the fold and seam axes must differ");
-  if (hi != 1) return xg_fail(XG_EINVAL, std::string(who) + ": the fold is the upper halo: hi must be 1");
-  if (skip < 0 || skip > 1) return xg_fail(XG_EINVAL, std::string(who) + ": skip must be 0 or 1");
-  if (shape[axis] - skip < 1)
-    return xg_fail(XG_EINVAL, std::string(who) + ": halo width exceeds the interior rows of the fold axis");
-  if (period < 1) return xg_fail(XG_EINVAL, std::string(who) + ": period must be positive");
-  for (int64_t k = 0; k < shape[seam_axis]; ++k) {  // the check xg_fold_rows makes, before any CUDA call
-    int64_t src = (mirror - k) % period;
-    if (src < 0) src += period;
-    if (src >= shape[seam_axis])
-      return xg_fail(XG_ENOTIMPL, std::string(who) + ": seam position incompatible with the pivot: the mirror "
-                                                     "partner of a seam index lies outside the seam dim");
-  }
   HaloStage h;
   h.kind = kHaloFold;
   h.seam_axis = seam_axis;
@@ -588,6 +641,43 @@ extern "C" int xg_host_workspace_bytes(int device, int64_t* bytes) {
   if (!w) return XG_OK;
   std::lock_guard<std::mutex> lock(w->mu);
   *bytes = (int64_t)(kSlots * (w->slab_in_bytes + w->slab_out_bytes + w->partner_bytes) + w->metric_bytes[0] +
-                     w->metric_bytes[1] + 2 * w->halo_bytes + w->const_bytes);
+                     w->metric_bytes[1] + w->metric_bytes[2] + 2 * w->halo_bytes + w->const_bytes);
   return XG_OK;
+}
+
+extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
+                                    int op_a, int lo_a, int hi_a, int bc_a, double fill_a, const void* pre_a,
+                                    const int64_t* pre_a_strides, int axis_b, int op_b, int lo_b, int hi_b, int bc_b,
+                                    double fill_b, const void* pre_b, const int64_t* pre_b_strides, int subtract,
+                                    const void* post, const int64_t* post_strides, int device) {
+  const PairTerm t{b, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, subtract};
+  const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
+               pre_b, pre_b_strides, post, post_strides, device, &t};
+  int rc = validate_pair_call("xg_stencil_pair_host", c);
+  if (rc) return rc;
+  return run_slabs(c, HaloStage{});
+}
+
+extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, void* out, int ndim,
+                                         const int64_t* shape, int op_a, int lo_a, int hi_a, int bc_a, double fill_a,
+                                         const void* pre_a, const int64_t* pre_a_strides, int axis_b, int op_b,
+                                         int lo_b, int hi_b, int bc_b, double fill_b, const void* pre_b,
+                                         const int64_t* pre_b_strides, int subtract, const void* post,
+                                         const int64_t* post_strides, int seam_axis, int skip, int64_t mirror,
+                                         int64_t period, int negate, int device) {
+  const char* who = "xg_stencil_pair_host_fold";
+  const PairTerm t{b, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, subtract};
+  const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
+               pre_b, pre_b_strides, post, post_strides, device, &t};
+  int rc = validate_pair_call(who, c);
+  if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
+  if (rc) return rc;
+  HaloStage h;
+  h.kind = kHaloFold;
+  h.seam_axis = seam_axis;
+  h.skip = skip;
+  h.mirror = mirror;
+  h.period = period;
+  h.negate = negate ? 1 : 0;
+  return run_slabs(c, h);
 }

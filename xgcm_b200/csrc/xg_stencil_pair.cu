@@ -12,6 +12,9 @@
 //     ta = OPa(A x ma), tb = OPb(B x mb), s = ta +- tb, out = s / post   — each rounded to the field dtype.
 // Both stencils are length preserving (lo + hi == 1: center <-> left / right), so A, B and out share one shape.
 //
+// xg_stencil_pair_halo takes optional halo planes of the B term (the folded north row of a tripolar grid): padB
+// reads them instead of the boundary rule on their side, here and in the tile kernel (XgTileSpec::halo_lo / hi).
+//
 // Work split: a warp owns 32 x VEC contiguous cells of the innermost dim and marches J
 // cells along axis b keeping B's previous row in registers; the x-neighbour of A comes from a warp shuffle,
 // only the lanes at a warp or row edge do one extra scalar load (or take the boundary value).
@@ -34,6 +37,8 @@ struct PairArgs {
   int op_a, lo_a, bc_a;          // hi_a = 1 - lo_a
   int op_b, lo_b, bc_b;
   T fill_a, fill_b;
+  const T* halo_lo;  // optional planes (outer, inner) of B x mb replacing bc_b below row 0 / above row nb - 1
+  const T* halo_hi;
   int subtract;
   XgOperand ma, mb, post;  // broadcast operands laid out against the common shape, collapsed around axis b
   int J;
@@ -163,10 +168,12 @@ __global__ void __launch_bounds__(kThreads, 3) k_stencil_pair(const PairArgs<T> 
     }
     return v;
   };
-  // padded row k of B (k in [0, nb]): source row k - lo_b, with the boundary rule at the two ends
+  // padded row k of B (k in [0, nb]): source row k - lo_b, with the halo plane or the boundary rule at the two ends
   auto padB = [&](int64_t k) -> Pack {
     const int64_t s = k - p.lo_b;
     if (s >= 0 && s < p.nb) return loadB(s);
+    const T* halo = s < 0 ? p.halo_lo : p.halo_hi;
+    if (halo) return xg_ld_cached<T, VEC>(halo + o * p.inner + i);
     if (p.bc_b == XG_BC_FILL) {
       Pack r;
 #pragma unroll
@@ -257,7 +264,7 @@ template <typename T>
 int pair_typed(const void* a, const void* b, void* out, int ndim, const int64_t* shape, int op_a, int lo_a, int bc_a,
                double fill_a, const void* pre_a, const int64_t* pre_a_strides, int axis_b, int op_b, int lo_b, int bc_b,
                double fill_b, const void* pre_b, const int64_t* pre_b_strides, int subtract, const void* post,
-               const int64_t* post_strides, cudaStream_t st) {
+               const int64_t* post_strides, const void* halo_lo_b, const void* halo_hi_b, cudaStream_t st) {
   constexpr int VEC = XgVecWidth<T>::value;
   XgView v;
   int rc = xg_collapse_view(ndim, shape, axis_b, &v);
@@ -278,10 +285,13 @@ int pair_typed(const void* a, const void* b, void* out, int ndim, const int64_t*
   p.bc_b = bc_b;
   p.fill_a = static_cast<T>(fill_a);
   p.fill_b = static_cast<T>(fill_b);
+  p.halo_lo = static_cast<const T*>(halo_lo_b);
+  p.halo_hi = static_cast<const T*>(halo_hi_b);
   p.subtract = subtract;
   if (v.n == 0 || p.nx == 0) return xg_fail(XG_EINVAL, "xg_stencil_pair: empty operated axis");
   if (v.outer == 0 || v.inner == 0) return XG_OK;
-  bool vec_ok = p.nx % VEC == 0 && ((uintptr_t)a % 16 == 0) && ((uintptr_t)b % 16 == 0) && ((uintptr_t)out % 16 == 0);
+  bool vec_ok = p.nx % VEC == 0 &&
+                (((uintptr_t)a | (uintptr_t)b | (uintptr_t)out | (uintptr_t)halo_lo_b | (uintptr_t)halo_hi_b) % 16 == 0);
   const int vec = vec_ok ? VEC : 1;
   rc = xg_make_operand(pre_a, pre_a_strides, ndim, shape, axis_b, vec, sizeof(T), &p.ma, "xg_stencil_pair(pre_a)");
   if (rc) return rc;
@@ -308,7 +318,8 @@ int pair_typed(const void* a, const void* b, void* out, int ndim, const int64_t*
     ts.hi_b = 1 - p.lo_b;
     ts.bc_b = p.bc_b;
     ts.fill_b = p.fill_b;
-    ts.halo_lo = ts.halo_hi = nullptr;
+    ts.halo_lo = p.halo_lo;
+    ts.halo_hi = p.halo_hi;
     ts.subtract = p.subtract;
     ts.out = p.out;
     if (xg_tile_operand_from<T>(p.ma, p.outer, p.inner, &ts.ma) && xg_tile_operand_from<T>(p.mb, p.outer, p.inner, &ts.mb) &&
@@ -322,13 +333,12 @@ int pair_typed(const void* a, const void* b, void* out, int ndim, const int64_t*
   return launch_pair<T, 1>(p, st);
 }
 
-}  // namespace
-
-extern "C" int xg_stencil_pair(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
-                               int op_a, int lo_a, int hi_a, int bc_a, double fill_a, const void* pre_a,
-                               const int64_t* pre_a_strides, int axis_b, int op_b, int lo_b, int hi_b, int bc_b,
-                               double fill_b, const void* pre_b, const int64_t* pre_b_strides, int subtract,
-                               const void* post, const int64_t* post_strides, void* stream) {
+// the checks and dtype dispatch of both entry points
+int pair_entry(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape, int op_a, int lo_a,
+               int hi_a, int bc_a, double fill_a, const void* pre_a, const int64_t* pre_a_strides, int axis_b, int op_b,
+               int lo_b, int hi_b, int bc_b, double fill_b, const void* pre_b, const int64_t* pre_b_strides,
+               int subtract, const void* post, const int64_t* post_strides, const void* halo_lo_b,
+               const void* halo_hi_b, void* stream) {
   if (!a || !b || !out || !shape) return xg_fail(XG_EINVAL, "xg_stencil_pair: null pointer");
   if (ndim < 2 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, "xg_stencil_pair: needs 2 <= ndim <= XG_MAX_NDIM");
   if (axis_b < 0 || axis_b >= ndim - 1)
@@ -344,12 +354,37 @@ extern "C" int xg_stencil_pair(int dtype, const void* a, const void* b, void* ou
     return xg_fail(XG_EINVAL, "xg_stencil_pair: metric strides missing");
   if (subtract < 0 || subtract > 2) return xg_fail(XG_EINVAL, "xg_stencil_pair: subtract must be 0, 1 or 2");
   if (a == out || b == out) return xg_fail(XG_EINVAL, "xg_stencil_pair: in-place operation is not supported");
+  if ((halo_lo_b && halo_lo_b == out) || (halo_hi_b && halo_hi_b == out))
+    return xg_fail(XG_EINVAL, "xg_stencil_pair: a halo plane may not be the output");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (dtype == XG_F32)
     return pair_typed<float>(a, b, out, ndim, shape, op_a, lo_a, bc_a, fill_a, pre_a, pre_a_strides, axis_b, op_b, lo_b,
-                             bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, st);
+                             bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, halo_lo_b, halo_hi_b, st);
   if (dtype == XG_F64)
     return pair_typed<double>(a, b, out, ndim, shape, op_a, lo_a, bc_a, fill_a, pre_a, pre_a_strides, axis_b, op_b, lo_b,
-                              bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, st);
+                              bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, halo_lo_b, halo_hi_b, st);
   return xg_fail(XG_EINVAL, "xg_stencil_pair: dtype must be XG_F32 or XG_F64");
+}
+
+}  // namespace
+
+extern "C" int xg_stencil_pair(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
+                               int op_a, int lo_a, int hi_a, int bc_a, double fill_a, const void* pre_a,
+                               const int64_t* pre_a_strides, int axis_b, int op_b, int lo_b, int hi_b, int bc_b,
+                               double fill_b, const void* pre_b, const int64_t* pre_b_strides, int subtract,
+                               const void* post, const int64_t* post_strides, void* stream) {
+  return pair_entry(dtype, a, b, out, ndim, shape, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, axis_b, op_b,
+                    lo_b, hi_b, bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, nullptr, nullptr,
+                    stream);
+}
+
+extern "C" int xg_stencil_pair_halo(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
+                                    int op_a, int lo_a, int hi_a, int bc_a, double fill_a, const void* pre_a,
+                                    const int64_t* pre_a_strides, int axis_b, int op_b, int lo_b, int hi_b, int bc_b,
+                                    double fill_b, const void* pre_b, const int64_t* pre_b_strides, int subtract,
+                                    const void* post, const int64_t* post_strides, const void* halo_lo_b,
+                                    const void* halo_hi_b, void* stream) {
+  return pair_entry(dtype, a, b, out, ndim, shape, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, axis_b, op_b,
+                    lo_b, hi_b, bc_b, fill_b, pre_b, pre_b_strides, subtract, post, post_strides, halo_lo_b, halo_hi_b,
+                    stream);
 }

@@ -191,6 +191,9 @@ __global__ void __launch_bounds__(kConsumers + 32, HAS_A ? 2 : 3)  // the pair's
     const int x = x0 + vxs * VEC, prow = p0 + ty;
     const int prc = prow < Po ? prow : (int)Po - 1;  // clamped row for the scalar metric loads of spare rows
     const bool act = vx < NVR && x < n && prow < Po;
+    // slots past the row end in the last x tile: their direct global loads (halo planes, wrap rows) read the
+    // row's last vector instead of cells past the end of the plane / array; nothing of theirs is stored
+    const int xl = x < n ? x : (int)n - VEC;
     const int nz = (s.Zn - z0 < U) ? (int)(s.Zn - z0) : U;
     const unsigned char* st = stage0 + (size_t)b * a.stage_bytes;
     const T* As = reinterpret_cast<const T*>(st) + ia;
@@ -278,16 +281,16 @@ __global__ void __launch_bounds__(kConsumers + 32, HAS_A ? 2 : 3)  // the pair's
       if (low_b || high_b) {
         // (B x mb)[z, row, x .. x + VEC) from global memory: wrap-around and extrapolation partners
         auto Brow = [&](int64_t row) -> Pack {
-          Pack r = xg_ld_cached<T, VEC>(s.b + z * bsz + row * fsp + x);
+          Pack r = xg_ld_cached<T, VEC>(s.b + z * bsz + row * fsp + xl);
           if (mb_mode != M_NONE) {
 #pragma unroll
             for (int kk = 0; kk < VEC; ++kk)
-              r.v[kk] = r.v[kk] * __ldg(s.mb.ptr + z * s.mb.sz + row * s.mb.sp + (int64_t)(x + kk) * s.mb.sx);
+              r.v[kk] = r.v[kk] * __ldg(s.mb.ptr + z * s.mb.sz + row * s.mb.sp + (int64_t)(xl + kk) * s.mb.sx);
           }
           return r;
         };
         if (low_b) {  // s0 == -1
-          if (s.halo_lo) b0 = xg_ld_cached<T, VEC>(s.halo_lo + z * n + x);
+          if (s.halo_lo) b0 = xg_ld_cached<T, VEC>(s.halo_lo + z * n + xl);
           else if (s.bc_b == XG_BC_FILL) {
 #pragma unroll
             for (int kk = 0; kk < VEC; ++kk) b0.v[kk] = s.fill_b;
@@ -300,7 +303,7 @@ __global__ void __launch_bounds__(kConsumers + 32, HAS_A ? 2 : 3)  // the pair's
           }
         }
         if (high_b) {  // s1 == Pb
-          if (s.halo_hi) b1 = xg_ld_cached<T, VEC>(s.halo_hi + z * n + x);
+          if (s.halo_hi) b1 = xg_ld_cached<T, VEC>(s.halo_hi + z * n + xl);
           else if (s.bc_b == XG_BC_FILL) {
 #pragma unroll
             for (int kk = 0; kk < VEC; ++kk) b1.v[kk] = s.fill_b;

@@ -702,9 +702,15 @@ class Grid:
         "sub" (term a minus term b).  Anything the fused kernel does not cover runs as the explicit chain.
 
         ``_components``: the vector-component axes of ``da_a`` / ``da_b`` (divergence, vorticity); a term
-        across a north fold then folds its input as that component, which changes its sign."""
+        across a north fold then folds its input as that component, which changes its sign.
+
+        On a fold grid the term along the non-innermost dim may cross the fold: its folded row is the kernel's
+        halo plane (one ``xg_fold_rows`` launch beside the pair).  Numpy fields with a batch dim in front of
+        the operated (and seam) dims stream through the GPU in slabs (``xg_stencil_pair_host``)."""
         from . import ops
         from .device import as_device_tensor, result_like
+        from .grid_ufunc import _host_stream_route, _is_host_float, _merge_leading
+        from .padding import _axis_dim, _fold_plan, fold_halo_planes
 
         if combine not in ("add", "sub"):
             raise ValueError(f"combine must be 'add' or 'sub', got {combine!r}")
@@ -756,11 +762,11 @@ class Grid:
             in_dim = self.axes[ax_name].coords[from_pos]
             out_dim = self.axes[ax_name].coords.get(to_pos)
             folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
-            if folded or out_dim is None or lo + hi != 1 or pad_mode not in ("periodic", "fill", "extend"):
+            if out_dim is None or lo + hi != 1 or pad_mode not in ("periodic", "fill", "extend"):
                 return chain()
             fv = fills[ax_name] if fills[ax_name] is not None else 0.0
             terms.append(dict(op=funcname, lo=lo, hi=hi, pad=pad_mode, fill=fv, axn=da.get_axis_num(in_dim),
-                              in_dim=in_dim, out_dim=out_dim, ax=ax_name))
+                              in_dim=in_dim, out_dim=out_dim, ax=ax_name, folded=folded))
         ta, tb = terms
         out_dims_a = tuple(ta["out_dim"] if d == ta["in_dim"] else d for d in da_a.dims)
         out_dims_b = tuple(tb["out_dim"] if d == tb["in_dim"] else d for d in da_b.dims)
@@ -778,23 +784,61 @@ class Grid:
             return chain()  # neither (or both) terms act on the innermost dim
         host = not da_a.is_device
         dev = self._device_for(da_a)
+        # the kernel takes halo planes for the term along the strided dim only; the fold plane and the host twins
+        # are CUDA launches (as in grid_ufunc._apply_fused_stencil, a fold off a CUDA device keeps the chain)
+        if first["folded"] or (second["folded"] and dev.type != "cuda"):
+            return chain()
+        spec_a = (first["op"], first["lo"], first["hi"], first["pad"], first["fill"])
+        spec_b = (second["axn"], second["op"], second["lo"], second["hi"], second["pad"], second["fill"])
+        negate = _components is not None  # a vector component changes sign across the fold
+        probe = DataArray.__new__(DataArray)
+        probe._dims = out_dims_a
+
+        def finish(data):
+            res = DataArray(data, dims=out_dims_a, name=da_a.name)
+            res = _reattach_coords([res], self, None, {ta["out_dim"], tb["out_dim"]}, [da_a, da_b])[0]
+            return self._wrap_out(res, as_xarray)
+
+        if host and dev.type == "cuda" and _is_host_float(fa) and _is_host_float(fb) and fa.data.dtype == fb.data.dtype:
+            # numpy fields: slabs of the leading batch dims H2D -> xg_stencil_pair_halo -> D2H
+            dims, shape, dt = tuple(fb.dims), list(fb.shape), fa.data.dtype
+            pre_a = self._metric_host(self.get_metric(fa, ma_ax), fa.dims, dt) if ma_ax else None
+            pre_b = self._metric_host(self.get_metric(fb, mb_ax), fb.dims, dt) if mb_ax else None
+            post = self._metric_host(self.get_metric(probe, divide_by), out_dims_a, dt) if divide_by else None
+            core = [second["in_dim"], dims[-1]]
+            if second["folded"]:
+                core.append(_axis_dim(self, dims, self._folds[second["ax"]]["seam_axis"]))
+            route = _host_stream_route("pair", dims, shape, core, 0, 1,
+                                       operand_shapes=[m.shape for m in (pre_a, pre_b, post) if m is not None])
+            if route is not None:
+                _, ndrop, nmerge = route
+                shift = ndrop + nmerge - 1  # dims before the operated ones that the cut removes
+
+                def cut(a):
+                    return None if a is None else _merge_leading(a, ndrop, nmerge)
+
+                kw = dict(pre_a=cut(pre_a), pre_b=cut(pre_b), post=cut(post), device=dev.index)
+                spec_b = (spec_b[0] - shift,) + spec_b[1:]
+                if second["folded"]:
+                    _, seam, skip, mirror, period = _fold_plan(self, second["ax"], dims, shape, 1)
+                    y = ops.stencil_pair_host_fold(cut(fa.data), cut(fb.data), spec_a, spec_b, seam - shift, skip,
+                                                   mirror, period, sub, negate=negate, **kw)
+                else:
+                    y = ops.stencil_pair_host(cut(fa.data), cut(fb.data), spec_a, spec_b, sub, **kw)
+                return finish(y.reshape(shape))
         xa, _ = as_device_tensor(fa.data, dev)
         xb, _ = as_device_tensor(fb.data, dev)
         if xa.dtype != xb.dtype:
             return chain()
         pre_a = self._metric_tensor(self.get_metric(fa, ma_ax), fa.dims, xa) if ma_ax else None
         pre_b = self._metric_tensor(self.get_metric(fb, mb_ax), fb.dims, xb) if mb_ax else None
-        post = None
-        if divide_by:
-            probe = DataArray.__new__(DataArray)
-            probe._dims = out_dims_a
-            post = self._metric_tensor(self.get_metric(probe, divide_by), out_dims_a, xa)
-        y = ops.stencil_pair(xa, xb, (first["op"], first["lo"], first["hi"], first["pad"], first["fill"]),
-                             (second["axn"], second["op"], second["lo"], second["hi"], second["pad"], second["fill"]),
-                             sub, pre_a=pre_a, pre_b=pre_b, post=post)
-        res = DataArray(result_like(y, host), dims=out_dims_a, name=da_a.name)
-        res = _reattach_coords([res], self, None, {ta["out_dim"], tb["out_dim"]}, [da_a, da_b])[0]
-        return self._wrap_out(res, as_xarray)
+        post = self._metric_tensor(self.get_metric(probe, divide_by), out_dims_a, xa) if divide_by else None
+        halo = {}
+        if second["folded"]:
+            halo["halo_lo_b"], halo["halo_hi_b"] = fold_halo_planes(self, second["ax"], fb.dims, xb, second["lo"],
+                                                                    second["pad"], pre=pre_b, negate=negate)
+        y = ops.stencil_pair(xa, xb, spec_a, spec_b, sub, pre_a=pre_a, pre_b=pre_b, post=post, **halo)
+        return finish(result_like(y, host))
 
     def divergence(self, u, v, axis_u="X", axis_v="Y", **kwargs):
         """Finite-volume horizontal divergence ``(diff(u * dy, X) + diff(v * dx, Y)) / area`` on a C-grid, metrics

@@ -603,7 +603,7 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             op, da, da if raw_arg is None else raw_arg, other_component, grid, ax_name, in_dim,
             out_dim, padding_width_real, padding, fill_value, pre_metric, post_metric_fn,
         )
-    from .padding import fold_edges, fold_halo_plane
+    from .padding import fold_edges, fold_halo_planes
 
     lo, hi = padding_width_real.get(ax_name, (0, 0))
     paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
@@ -661,11 +661,9 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
     post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
     halo_lo = halo_hi = None
     if folded:
-        # the north halo is the folded row (of x * pre, sign-flipped for a vector component); a periodic
-        # south edge wraps the row above the top, which is that same fold row (reference padding.py:723-762)
-        halo_hi = fold_halo_plane(grid, ax_name, da.dims, x, pre=pre_t, negate=isinstance(raw_arg, dict))
-        if lo and ax_padding == "periodic":
-            halo_lo = halo_hi
+        # the north halo is the folded row of x * pre, sign-flipped for a vector component
+        halo_lo, halo_hi = fold_halo_planes(grid, ax_name, da.dims, x, lo, ax_padding, pre=pre_t,
+                                            negate=isinstance(raw_arg, dict))
     out = ops.stencil2(x, axis_num, op, lo, hi, bc, fv, pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
     return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
 
@@ -677,15 +675,15 @@ def _is_host_float(da) -> bool:
 def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_ok=True, operand_shapes=()):
     """Whether a numpy field streams through a host slab pipeline, and how it is cut.
 
-    ``kind``: "plain" (``xg_stencil2_host``), "fold" (the operator crosses a north fold) or "connected" (face
-    connections); ``core_dims``: the dims the operator or any halo source indexes (operated dim; seam dim;
-    face dim and the dims of the connection axes).  The slabs are cut along dim 0: leading size-1 dims are
-    dropped first, then the leading batch dims (those before the first core dim) are merged into one dim 0
-    -- as far as every broadcast operand (metric ``operand_shapes``, 1 where it broadcasts) merges with them.
-    A plain grid cuts the field's own dim 0 (no merge), which may be the operated dim.  Returns ``(kind,
-    dims dropped, dims merged)``, or None for the whole-field device path: a fold or connected field with no
-    batch dim in front, a halo wider than one cell, a pre-metric or a partner component that cannot stream
-    beside the field on a connected grid."""
+    ``kind``: "plain" (``xg_stencil2_host``), "fold" (the operator crosses a north fold), "connected" (face
+    connections) or "pair" (``xg_stencil_pair_host`` and its fold variant); ``core_dims``: the dims the
+    operator or any halo source indexes (operated dims; seam dim; face dim and the dims of the connection
+    axes).  The slabs are cut along dim 0: leading size-1 dims are dropped first, then the leading batch dims
+    (those before the first core dim) are merged into one dim 0 -- as far as every broadcast operand (metric
+    ``operand_shapes``, 1 where it broadcasts) merges with them.  A plain grid cuts the field's own dim 0 (no
+    merge), which may be the operated dim.  Returns ``(kind, dims dropped, dims merged)``, or None for the
+    whole-field device path: a fold, connected or pair field with no batch dim in front, a halo wider than
+    one cell, a pre-metric or a partner component that cannot stream beside the field on a connected grid."""
     first = min(list(dims).index(d) for d in core_dims)
     ndrop = 0
     while ndrop < first and shape[ndrop] == 1:

@@ -676,37 +676,118 @@ def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int,
     return out
 
 
+def _pair_specs(spec_a, spec_b, ndim: int):
+    """C-ABI values of the two terms of a pair: ``(op_a, lo_a, hi_a, bc_a, fill_a)``, ``(axis_b, op_b, lo_b, hi_b,
+    bc_b, fill_b)``."""
+    op_a, lo_a, hi_a, pad_a, fill_a = spec_a
+    axis_b, op_b, lo_b, hi_b, pad_b, fill_b = spec_b
+    for pad_ in (pad_a, pad_b):
+        if pad_ not in ("periodic", "fill", "extend"):
+            raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'], but got {pad_}")
+    return ((_capi.OPS[op_a], int(lo_a), int(hi_a), _capi.BCS[pad_a], float(0.0 if fill_a is None else fill_a)),
+            (_norm_axis(axis_b, ndim), _capi.OPS[op_b], int(lo_b), int(hi_b), _capi.BCS[pad_b],
+             float(0.0 if fill_b is None else fill_b)))
+
+
 def stencil_pair(a: torch.Tensor, b: torch.Tensor, spec_a, spec_b, subtract: int = 0,
                  pre_a: Optional[torch.Tensor] = None, pre_b: Optional[torch.Tensor] = None,
-                 post: Optional[torch.Tensor] = None) -> torch.Tensor:
+                 post: Optional[torch.Tensor] = None, halo_lo_b: Optional[torch.Tensor] = None,
+                 halo_hi_b: Optional[torch.Tensor] = None) -> torch.Tensor:
     """``(OPa(a * pre_a) along the innermost dim  +|-  OPb(b * pre_b) along another dim) / post`` in one pass
-    (``xg_stencil_pair``).  ``spec_a = (op, lo, hi, padding, fill)`` acts on the LAST dim, ``spec_b =
-    (axis, op, lo, hi, padding, fill)`` on ``axis`` != last.  All arrays share ``a``'s shape; metrics broadcast."""
+    (``xg_stencil_pair_halo``).  ``spec_a = (op, lo, hi, padding, fill)`` acts on the LAST dim, ``spec_b =
+    (axis, op, lo, hi, padding, fill)`` on ``axis`` != last.  All arrays share ``a``'s shape; metrics broadcast.
+
+    ``halo_lo_b`` / ``halo_hi_b``: optional planes (``a``'s shape with extent 1 along ``axis``, already
+    weighted by ``pre_b``) that pad the term along ``axis`` instead of its padding on their side, e.g. the
+    folded north row of :func:`fold_rows`."""
     lib = _capi.load()
     _require_cuda(a, "field a")
     _require_cuda(b, "field b")
     if a.shape != b.shape or a.dtype != b.dtype:
         raise ValueError("stencil_pair: both fields must have the same shape and dtype")
     a, b = a.contiguous(), b.contiguous()
-    op_a, lo_a, hi_a, pad_a, fill_a = spec_a
-    axis_b, op_b, lo_b, hi_b, pad_b, fill_b = spec_b
-    axis_b = _norm_axis(axis_b, a.dim())
-    for pad_ in (pad_a, pad_b):
-        if pad_ not in ("periodic", "fill", "extend"):
-            raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'], but got {pad_}")
+    term_a, term_b = _pair_specs(spec_a, spec_b, a.dim())
     shape = list(a.shape)
     out = torch.empty_like(a)
     k1, pa_ptr, pa_st = _operand(pre_a, shape, a, "pre metric a")
     k2, pb_ptr, pb_st = _operand(pre_b, shape, a, "pre metric b")
     k3, po_ptr, po_st = _operand(post, shape, a, "post metric")
+    plane = int(np.prod([s for d, s in enumerate(shape) if d != term_b[0]], dtype=np.int64))
+    halos = []
+    for h, what in ((halo_lo_b, "halo_lo_b"), (halo_hi_b, "halo_hi_b")):
+        if h is not None:
+            _require_cuda(h, what)
+            if h.device != a.device:
+                raise RuntimeError(f"{what} is on {h.device}, field on {a.device}")
+            h = h.to(a.dtype).contiguous()
+            if h.numel() != plane:
+                raise ValueError(f"{what} has wrong size")
+        halos.append(h)
     if out.numel():
         with torch.cuda.device(a.device):
-            rc = lib.xg_stencil_pair(
+            rc = lib.xg_stencil_pair_halo(
                 _dtype_code(a), a.data_ptr(), b.data_ptr(), out.data_ptr(), a.dim(), _capi.i64_array(shape),
-                _capi.OPS[op_a], lo_a, hi_a, _capi.BCS[pad_a], float(0.0 if fill_a is None else fill_a), pa_ptr, pa_st,
-                axis_b, _capi.OPS[op_b], lo_b, hi_b, _capi.BCS[pad_b], float(0.0 if fill_b is None else fill_b),
-                pb_ptr, pb_st, int(subtract), po_ptr, po_st, _stream_ptr(a))
+                *term_a, pa_ptr, pa_st, *term_b, pb_ptr, pb_st, int(subtract), po_ptr, po_st,
+                *[None if h is None else h.data_ptr() for h in halos], _stream_ptr(a))
         _capi.check(rc)
+    return out
+
+
+def _host_pair_prep(a, b, spec_a, spec_b, pre_a, pre_b, post, out, device, what):
+    """Checks and buffers shared by the host pair twins: (a, b, shape, C-ABI term values, the three operands,
+    out, device index)."""
+    for x in (a, b):
+        if not isinstance(x, np.ndarray):
+            raise TypeError(f"{what} takes numpy arrays")
+    if not torch.cuda.is_available():
+        raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
+    if a.shape != b.shape or a.dtype != b.dtype:
+        raise ValueError(f"{what}: both fields must have the same shape and dtype")
+    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
+    term_a, term_b = _pair_specs(spec_a, spec_b, a.ndim)
+    shape = list(a.shape)
+    if out is None:
+        out = pinned_empty(shape, a.dtype)
+    elif list(out.shape) != shape or out.dtype != a.dtype or not out.flags.c_contiguous:
+        raise ValueError("out has wrong shape/dtype/layout")
+    ops_ = [_host_operand(m, shape, a.dtype, w) for m, w in ((pre_a, "pre metric a"), (pre_b, "pre metric b"),
+                                                             (post, "post metric"))]
+    dev = torch.cuda.current_device() if device is None else int(device)
+    return a, b, shape, term_a, term_b, ops_, out, dev
+
+
+def stencil_pair_host(a: np.ndarray, b: np.ndarray, spec_a, spec_b, subtract: int = 0,
+                      pre_a: Optional[np.ndarray] = None, pre_b: Optional[np.ndarray] = None,
+                      post: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
+                      device: Optional[int] = None) -> np.ndarray:
+    """Host-buffer twin of :func:`stencil_pair` (``xg_stencil_pair_host``): ``a`` and ``b`` stream through the
+    GPU in slabs of dim 0, which must be a batch dim (not ``spec_b``'s axis)."""
+    lib = _capi.load()
+    a, b, shape, term_a, term_b, (pa, pb, po), out, dev = _host_pair_prep(a, b, spec_a, spec_b, pre_a, pre_b, post,
+                                                                           out, device, "stencil_pair_host")
+    rc = lib.xg_stencil_pair_host(
+        _capi.dtype_code(a.dtype), a.ctypes.data, b.ctypes.data, out.ctypes.data, a.ndim, _capi.i64_array(shape),
+        *term_a, pa[1], pa[2], *term_b, pb[1], pb[2], int(subtract), po[1], po[2], dev)
+    _capi.check(rc)
+    return out
+
+
+def stencil_pair_host_fold(a: np.ndarray, b: np.ndarray, spec_a, spec_b, seam_axis: int, skip: int, mirror: int,
+                           period: int, subtract: int = 0, negate: bool = False, pre_a: Optional[np.ndarray] = None,
+                           pre_b: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None,
+                           out: Optional[np.ndarray] = None, device: Optional[int] = None) -> np.ndarray:
+    """:func:`stencil_pair_host` with the term along ``spec_b``'s axis across a north fold
+    (``xg_stencil_pair_host_fold``): each slab's ``halo_hi_b`` is the folded row of ``b * pre_b``
+    (:func:`fold_rows` with ``seam_axis, skip, mirror, period, negate``), also ``halo_lo_b`` when ``spec_b``
+    pads the south edge periodically.  Dim 0 must be neither ``spec_b``'s axis nor ``seam_axis``."""
+    lib = _capi.load()
+    a, b, shape, term_a, term_b, (pa, pb, po), out, dev = _host_pair_prep(a, b, spec_a, spec_b, pre_a, pre_b, post,
+                                                                           out, device, "stencil_pair_host_fold")
+    rc = lib.xg_stencil_pair_host_fold(
+        _capi.dtype_code(a.dtype), a.ctypes.data, b.ctypes.data, out.ctypes.data, a.ndim, _capi.i64_array(shape),
+        *term_a, pa[1], pa[2], *term_b, pb[1], pb[2], int(subtract), po[1], po[2], _norm_axis(seam_axis, a.ndim),
+        int(skip), int(mirror), int(period), 1 if negate else 0, dev)
+    _capi.check(rc)
     return out
 
 

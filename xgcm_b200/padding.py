@@ -171,6 +171,15 @@ def fold_halo_plane(grid, fold_axis: str, dims, x, pre=None, negate: bool = Fals
     return ops.fold_rows(x, f, s, 1, skip, mirror, period, negate=negate, pre=pre)
 
 
+def fold_halo_planes(grid, fold_axis: str, dims, x, lo: int, south, pre=None, negate: bool = False):
+    """``(halo_lo, halo_hi)`` of a one-cell stencil whose north edge crosses the fold of ``fold_axis``:
+    halo_hi is the folded row (:func:`fold_halo_plane`).  A periodic south edge wraps the row above the top,
+    which is that same fold row (reference padding.py:723-762), so it is halo_lo too when the stencil pads
+    the south edge (``lo``); otherwise halo_lo is None and the boundary condition ``south`` pads that edge."""
+    halo_hi = fold_halo_plane(grid, fold_axis, dims, x, pre=pre, negate=negate)
+    return (halo_hi if lo and south == "periodic" else None), halo_hi
+
+
 def _pad_fold(data, grid, padding_width, padding, fill_value):
     """Padding on a grid with a north fold (reference padding.py:687-762), on the device.
 
