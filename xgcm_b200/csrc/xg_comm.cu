@@ -235,7 +235,8 @@ int sharded_typed(XgComm* c, int op, const void* in, void* out, int ndim, const 
   if (rc) return rc;
   constexpr int VECW = XgVecWidth<T>::value;
   // 16-byte vectors along `inner` when every row start stays aligned (workspace slots are 256-byte aligned)
-  bool vec_ok = v.inner % VECW == 0 && ((uintptr_t)in % 16 == 0) && ((uintptr_t)out % 16 == 0);
+  bool vec_ok = v.inner % VECW == 0 && ((uintptr_t)in % 16 == 0) && ((uintptr_t)out % 16 == 0) &&
+                xg_vec_view_ok(pa.pre) && xg_vec_view_ok(pa.post);
   if (!vec_ok) {
     pa.pre.vec_ok = 0;
     pa.post.vec_ok = 0;

@@ -77,7 +77,13 @@ struct XgOperand {
   XgGroups inner;       // flat inner index -> element offset
   int inner_mode;       // XG_IM_*
   int vec_ok;           // CONTIG and every offset is a multiple of the vector width
+  int wide_span;        // GENERIC and the inner offsets span >= 2^31 elements: two elements of one vector
+                        // may lie further apart than XgOperandView's 32-bit deltas reach, so the
+                        // launchers take their VEC = 1 instance (no deltas) for such an operand
 };
+
+// an operand the VEC > 1 instances of the XgOperandView kernels can take (absent operands included)
+static inline bool xg_vec_view_ok(const XgOperand& m) { return !m.wide_span; }
 
 struct XgView {
   int64_t outer, n, inner;

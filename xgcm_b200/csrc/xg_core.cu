@@ -139,6 +139,13 @@ int xg_make_operand(const void* ptr, const int64_t* strides, int ndim,
     op->inner_mode = XG_IM_CONTIG;
   } else {
     op->inner_mode = XG_IM_GENERIC;
+    // offsets of the inner index lie in [0, span] (strides are non-negative), so any two differ by at most span
+    int64_t span = 0;
+    for (int k = 0; k < op->inner.n; ++k) {
+      const int64_t ext = (op->inner.size[k] - 1) * op->inner.stride[k];
+      span = (ext >= (1ll << 31) || span + ext >= (1ll << 31)) ? (1ll << 31) : span + ext;
+    }
+    op->wide_span = span >= (1ll << 31) ? 1 : 0;
   }
   op->vec_ok = 0;
   if (op->inner_mode == XG_IM_CONTIG && vec > 1) {

@@ -521,7 +521,8 @@ int scan_launch(ScanArgs<T>& a, cudaStream_t st) {
   constexpr int VEC = XgVecWidth<T>::value;
   constexpr int U = 8;
   if (a.inner > 1) {
-    bool vec_ok = (a.inner % VEC == 0) && ((uintptr_t)a.in % 16 == 0) && ((uintptr_t)a.out % 16 == 0);
+    bool vec_ok = (a.inner % VEC == 0) && ((uintptr_t)a.in % 16 == 0) && ((uintptr_t)a.out % 16 == 0) &&
+                  xg_vec_view_ok(a.pre) && xg_vec_view_ok(a.post);
     // few columns: prefer 4x more (scalar) threads over 16-byte accesses
     if (vec_ok && a.outer * (a.inner / VEC) < XG_SMS * 64) vec_ok = false;
     if (vec_ok) {

@@ -1011,7 +1011,8 @@ int dispatch_layout(StencilArgs<T>& a, cudaStream_t st) {
         }
       }
     }
-    if (ptr_ok && a.inner % VEC == 0) return launch_plane<T, VEC, OP, MET>(a, st);
+    if (ptr_ok && a.inner % VEC == 0 && xg_vec_view_ok(a.pre) && xg_vec_view_ok(a.post))
+      return launch_plane<T, VEC, OP, MET>(a, st);
     a.pre.vec_ok = 0;
     a.post.vec_ok = 0;
     return launch_plane<T, 1, OP, MET>(a, st);

@@ -329,7 +329,8 @@ int pair_typed(const void* a, const void* b, void* out, int ndim, const int64_t*
       if (rc || launched) return rc;
     }
   }
-  if (vec_ok) return launch_pair<T, VEC>(p, st);
+  if (vec_ok && xg_vec_view_ok(p.ma) && xg_vec_view_ok(p.mb) && xg_vec_view_ok(p.post))
+    return launch_pair<T, VEC>(p, st);
   return launch_pair<T, 1>(p, st);
 }
 

@@ -145,7 +145,8 @@ int reduce_launch(ReduceArgs<T>& a, cudaStream_t st) {
   constexpr int VEC = XgVecWidth<T>::value;
   constexpr int U = 8;
   if (a.inner > 1) {
-    bool vec_ok = (a.inner % VEC == 0) && ((uintptr_t)a.in % 16 == 0) && ((uintptr_t)a.out % 16 == 0);
+    bool vec_ok = (a.inner % VEC == 0) && ((uintptr_t)a.in % 16 == 0) && ((uintptr_t)a.out % 16 == 0) &&
+                  xg_vec_view_ok(a.w);
     if (vec_ok && a.outer * (a.inner / VEC) < XG_SMS * 64) vec_ok = false;
     a.nvec_inner = vec_ok ? a.inner / VEC : a.inner;
     if (!vec_ok) a.w.vec_ok = 0;
