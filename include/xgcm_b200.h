@@ -398,10 +398,11 @@ XG_API int xg_stencil2_host_multi(int nout, const int* op, int dtype, const void
 
 /*
  * Host-buffer twins of xg_cumscan / xg_wreduce / xg_vinterp_linear (same semantics, HOST pointers, `device`
- * instead of a stream; synchronous).  The field is streamed in slabs of the first NON-operated dimension
- * (strided 2-D copies when that is not dim 0), so every line along the operated axis stays whole: no
- * halo between slabs, summation order untouched.  Metric / weight / theta / target operands are uploaded
- * whole.  Replaces the host side of xgcm/grid.py:1316 (cumsum), :1598-1605 (integrate), :1680-1685
+ * instead of a stream; synchronous).  The field is streamed in slabs of a NON-operated dimension (the first
+ * one for cumscan / wreduce; see xg_vinterp_conservative_host for the transform twins), with strided 2-D
+ * copies when that is not dim 0, so every line along the operated axis stays whole: no halo between slabs,
+ * summation order untouched.  Metric / weight / target operands are uploaded whole; a dense theta field
+ * streams beside the field.  Replaces the host side of xgcm/grid.py:1316 (cumsum), :1598-1605 (integrate), :1680-1685
  * (average) and xgcm/transform.py:233-249 for numpy-backed fields.
  */
 XG_API int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,
@@ -416,6 +417,26 @@ XG_API int xg_vinterp_linear_host(int dtype, const void* phi, const void* theta,
                            const int64_t* target_strides, int64_t m, void* out, int ndim,
                            const int64_t* shape, int axis, int mask_edges, int bypass_checks,
                            int logarithmic, int device);
+
+/*
+ * Host-buffer twin of xg_vinterp_conservative (same semantics, HOST pointers, `device` instead of a stream;
+ * synchronous).  Replaces the host side of xgcm/transform.py:157-198 for numpy-backed fields.  The two transform
+ * twins (this and xg_vinterp_linear_host) cut slabs along the outermost non-operated dim of extent > 1 one index of
+ * which (phi, theta, theta-bounds scratch and result bytes together) fits the slab budget, else the innermost such
+ * dim; a dense theta field streams in the same slabs as phi, a broadcast one is uploaded whole.  theta_at_centers:
+ * theta holds n cell-centre values along `axis` (not n + 1 bounds); the bounds are made on the device by the
+ * center -> outer interp with extend padding, i.e. grid.interp(theta, axis, padding="extend") (transform.py:289-294).
+ * A zero-length axis gives all-NaN bins.  Every argument is checked before any CUDA call (XG_EINVAL).
+ */
+XG_API int xg_vinterp_conservative_host(int dtype, const void* phi, const void* theta,
+                                 const int64_t* theta_strides, int theta_at_centers,
+                                 const void* target_bins, int64_t m, int flip_out, void* out, int ndim,
+                                 const int64_t* shape, int axis, int device);
+
+/* Device bytes the workspace of xg_stencil2_host_multi, xg_cumscan_host, xg_wreduce_host and the two transform twins
+ * holds on `device` (slot buffers, theta-bounds scratch, aux operands); 0 before the first call or after
+ * xg_host_workspace_release. */
+XG_API int xg_host_pipe_workspace_bytes(int device, int64_t* bytes);
 
 /* Free the cached device slabs / streams of the *_host entry points. */
 XG_API int xg_host_workspace_release(void);

@@ -117,6 +117,11 @@ SIGNATURES = {
         [C.c_int, _vp, _vp, _i64p, _vp, _i64p, C.c_int64, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int,
          C.c_int, C.c_int],
     ),
+    "xg_vinterp_conservative_host": (
+        C.c_int,
+        [C.c_int, _vp, _vp, _i64p, C.c_int, _vp, C.c_int64, C.c_int, _vp, C.c_int, _i64p, C.c_int, C.c_int],
+    ),
+    "xg_host_pipe_workspace_bytes": (C.c_int, [C.c_int, _i64p]),
     "xg_host_workspace_release": (C.c_int, []),
     "xg_stencil_pair": (
         C.c_int,

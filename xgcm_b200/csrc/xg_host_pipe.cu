@@ -8,12 +8,24 @@
 //                            times (xgcm/grid.py:796-832 would re-read it per call).
 //   xg_cumscan_host          xgcm/grid.py:1306-1414 on numpy-backed fields
 //   xg_wreduce_host          xgcm/grid.py:1598-1605, :1680-1685
-//   xg_vinterp_linear_host   xgcm/transform.py:233-249
+//   xg_vinterp_linear_host        xgcm/transform.py:233-249
+//   xg_vinterp_conservative_host  xgcm/transform.py:157-198 (k_vconserv per slab)
 //
-// The three single-result twins cut slabs along the first NON-operated dimension: a slab of
-// (Z, y0:y1, X) is Z pieces of (y1-y0)*X contiguous elements -> one cudaMemcpy2DAsync each way.  Lines
-// along the operated axis stay whole, so no halo exchange between slabs is needed and summation order
-// is untouched.  Metric / weight / theta / target operands are small and uploaded whole, once.
+// Slabs are cut along a NON-operated dimension: a slab of (Z, y0:y1, X) is Z pieces of (y1-y0)*X
+// contiguous elements -> one cudaMemcpy2DAsync each way.  Lines along the operated axis stay whole, so
+// no halo exchange between slabs is needed and summation order is untouched.  xg_cumscan_host and
+// xg_wreduce_host cut the first non-operated dim, and upload their metric / weight whole, once.
+//
+// The two transform twins pick the outermost non-operated dim of extent > 1 one index of which (its phi,
+// theta, theta-bounds scratch and result bytes together) fits the slab budget, else the innermost one, so
+// that (time_counter=1, deptht, y, x) or a short time axis does not make one huge slab; the rows per slab
+// are sized from that same per-index total (the result of m >> n bins outweighs phi).  A dense theta field
+// is the pipe's second streamed input: it goes up in the same slab window as phi into its own per-slot
+// buffers.  A broadcast theta (a 1-D coordinate, (T, Z+1, 1, 1), ...) is uploaded whole once.  Theta given
+// at cell centres (xg_vinterp_conservative_host's theta_at_centers) becomes its n + 1 bounds on the device:
+// one xg_stencil2(interp, lo = hi = 1, extend) along the axis per slab into a per-slot scratch buffer (once,
+// into an aux buffer, for a broadcast theta) -- the center -> outer shift of grid.interp(theta, axis,
+// padding="extend"), so the bounds are the ones that call would give.
 //
 // Workspaces (device slabs, streams, events) are cached per device and guarded by a per-device mutex:
 // calls on different GPUs run concurrently, calls on one GPU serialise (they would fight for PCIe anyway).
@@ -36,6 +48,10 @@ struct PipeWorkspace {
   std::mutex mu;
   size_t in_cap[kSlots] = {0, 0, 0};
   void* d_in[kSlots] = {nullptr, nullptr, nullptr};
+  size_t in2_cap[kSlots] = {0, 0, 0};
+  void* d_in2[kSlots] = {nullptr, nullptr, nullptr};  // second streamed input (a dense theta field)
+  size_t scr_cap[kSlots] = {0, 0, 0};
+  void* d_scr[kSlots] = {nullptr, nullptr, nullptr};  // per-slab scratch (theta bounds made from centres)
   size_t out_cap[kSlots][kMaxOut] = {};
   void* d_out[kSlots][kMaxOut] = {};
   size_t aux_cap[kMaxAux] = {0, 0, 0, 0};
@@ -131,32 +147,57 @@ int copy_slab(void* dev, const void* host_base, const View3& v, int64_t j0, int6
   return XG_OK;
 }
 
-int64_t slab_rows(const View3& in, size_t es, int64_t extra_rows) {
+int64_t slab_budget_bytes() {
   int64_t target_bytes = 128ll << 20;
   if (const char* env = getenv("XG_HOST_SLAB_MB")) {  // tuning knob (benchmarks only)
     const long mb = atol(env);
     if (mb >= 1 && mb <= 4096) target_bytes = (int64_t)mb << 20;
   }
-  const int64_t row_bytes = (int64_t)(in.C * in.R * (int64_t)es);
-  int64_t rows = row_bytes > 0 ? target_bytes / row_bytes : in.L;
+  return target_bytes;
+}
+
+// rows of a slab dim of extent L whose one row (index) moves `row_bytes`
+int64_t slab_rows(int64_t L, int64_t row_bytes, int64_t extra_rows) {
+  int64_t rows = row_bytes > 0 ? slab_budget_bytes() / row_bytes : L;
   if (rows < 1) rows = 1;
-  if (rows > (in.L + 3) / 4) rows = (in.L + 3) / 4;  // at least 4 slabs when the dim allows: overlap
+  if (rows > (L + 3) / 4) rows = (L + 3) / 4;  // at least 4 slabs when the dim allows: overlap
   if (rows < 1 + extra_rows) rows = 1 + extra_rows;
   return rows;
 }
 
-// launch(j0, j1, i0, i1, d_in, d_out[], stream): kernels for output rows [j0, j1) given input rows [i0, i1)
-typedef std::function<int(int64_t, int64_t, int64_t, int64_t, void*, void* const*, cudaStream_t)> LaunchFn;
+// Optional parts of a pipeline: a second host input that goes up in the same slab window as the first, rows
+// [j0, j1) without halo, into per-slot buffers (its own [C][L][R] view, same L); a per-slot device scratch of
+// `scratch_row_bytes` per slab row; the bytes one slab row moves, which size the slabs (0: the first input's).
+struct PipeExtra {
+  const void* hin2 = nullptr;
+  View3 in2{0, 0, 0};
+  size_t scratch_row_bytes = 0;
+  int64_t row_bytes = 0;
+};
+
+struct SlabBufs {  // device buffers of the slot a slab runs in
+  void* in;
+  void* in2;      // the second input's rows, nullptr without one
+  void* scratch;  // nullptr without scratch
+  void* const* out;
+};
+
+// launch(j0, j1, i0, i1, bufs, stream): kernels for output rows [j0, j1) given input rows [i0, i1)
+typedef std::function<int(int64_t, int64_t, int64_t, int64_t, const SlabBufs&, cudaStream_t)> LaunchFn;
 
 // The pipeline.  `halo` = extra input rows wanted on each side of a slab (0, or 1 when some result is
 // operated along the slab dim).  Result k has view out[k] with the same L as the input.
 int run_pipe(PipeWorkspace* w, size_t es, const void* hin, const View3& in, int nout, void* const* hout,
-             const View3* out, int halo, const LaunchFn& launch) {
+             const View3* out, int halo, const LaunchFn& launch, const PipeExtra& ex = PipeExtra()) {
   if (in.L == 0 || in.C == 0 || in.R == 0) return XG_OK;
-  const int64_t rows = slab_rows(in, es, 0);
+  const int64_t rows = slab_rows(in.L, ex.row_bytes > 0 ? ex.row_bytes : in.C * in.R * (int64_t)es, 0);
   const int64_t nslab = xg_ceil_div(in.L, rows);
   for (int i = 0; i < kSlots; ++i) {
     int rc = ensure(&w->d_in[i], &w->in_cap[i], (size_t)(in.C * (rows + 2 * halo) * in.R) * es);
+    if (rc) return rc;
+    if (ex.hin2) rc = ensure(&w->d_in2[i], &w->in2_cap[i], (size_t)(ex.in2.C * rows * ex.in2.R) * es);
+    if (rc) return rc;
+    if (ex.scratch_row_bytes) rc = ensure(&w->d_scr[i], &w->scr_cap[i], ex.scratch_row_bytes * (size_t)rows);
     if (rc) return rc;
     for (int k = 0; k < nout; ++k) {
       rc = ensure(&w->d_out[i][k], &w->out_cap[i][k], (size_t)(out[k].C * rows * out[k].R) * es);
@@ -173,9 +214,13 @@ int run_pipe(PipeWorkspace* w, size_t es, const void* hin, const View3& in, int 
     }
     int rc = copy_slab(w->d_in[slot], hin, in, i0, i1, es, true, w->s_h2d);
     if (rc) return rc;
+    if (ex.hin2) rc = copy_slab(w->d_in2[slot], ex.hin2, ex.in2, j0, j1, es, true, w->s_h2d);
+    if (rc) return rc;
     XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
     XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[slot], 0));
-    rc = launch(j0, j1, i0, i1, w->d_in[slot], w->d_out[slot], w->s_k);
+    const SlabBufs bufs{w->d_in[slot], ex.hin2 ? w->d_in2[slot] : nullptr,
+                        ex.scratch_row_bytes ? w->d_scr[slot] : nullptr, w->d_out[slot]};
+    rc = launch(j0, j1, i0, i1, bufs, w->s_k);
     if (rc) {
       cudaDeviceSynchronize();
       return rc;
@@ -225,6 +270,183 @@ struct Session {  // device selected, workspace locked and initialised
 
 int first_free_dim(int ndim, int axis) { return (ndim == 1) ? -1 : (axis == 0 ? 1 : 0); }
 
+// ------------------------------------------------------------------- the two transform twins (theta beside phi)
+int64_t numel(int ndim, const int64_t* shape) {
+  int64_t n = 1;
+  for (int d = 0; d < ndim; ++d) n *= shape[d];
+  return n;
+}
+
+void dense_strides(int ndim, const int64_t* shape, int64_t* strides) {  // C order
+  int64_t s = 1;
+  for (int d = ndim - 1; d >= 0; --d) {
+    strides[d] = s;
+    s *= shape[d];
+  }
+}
+
+// theta is a dense C-contiguous array of `tshape` (dims of extent 1 aside): it streams beside phi
+bool theta_is_dense(int ndim, const int64_t* tshape, const int64_t* strides) {
+  int64_t ds[XG_MAX_NDIM];
+  dense_strides(ndim, tshape, ds);
+  for (int d = 0; d < ndim; ++d)
+    if (tshape[d] > 1 && strides[d] != ds[d]) return false;
+  return true;
+}
+
+// the compact shape of a broadcast theta: 1 where it is broadcast (stride 0) or of extent 1
+void compact_shape(int ndim, const int64_t* tshape, const int64_t* strides, int64_t* cshape) {
+  for (int d = 0; d < ndim; ++d) cshape[d] = (tshape[d] > 1 && strides[d] != 0) ? tshape[d] : 1;
+}
+
+// Slab dim of the transform twins: the outermost non-operated dim of extent > 1 whose one index -- its share of
+// `total_bytes` (phi, streamed theta, theta-bounds scratch and result together) -- fits the slab budget; else the
+// innermost non-operated dim of extent > 1; -1 when there is none (the whole field is one slab).
+int transform_slab_dim(int ndim, const int64_t* shape, int axis, int64_t total_bytes) {
+  const int64_t budget = slab_budget_bytes();
+  int inner = -1;
+  for (int d = 0; d < ndim; ++d) {
+    if (d == axis || shape[d] <= 1) continue;
+    if (total_bytes / shape[d] <= budget) return d;
+    inner = d;
+  }
+  return inner;
+}
+
+// theta of one transform-twin call: tshape = phi's shape with `tn` along the axis (n + 1 bounds, or n centres)
+struct ThetaPlan {
+  int dtype = XG_F32, ndim = 0, axis = 0, sd = -1;
+  size_t es = 4;
+  bool dense = false, centers = false;
+  int64_t tshape[XG_MAX_NDIM], bshape[XG_MAX_NDIM];  // theta as given; its n + 1 bounds
+  const void* d_bcast = nullptr;                     // broadcast theta's bounds on the device
+  int64_t bstrides[XG_MAX_NDIM];                     // and their strides
+
+  // bytes of the whole streamed theta and of the whole bounds scratch
+  int64_t stream_bytes() const { return dense ? numel(ndim, tshape) * (int64_t)es : 0; }
+  int64_t scratch_bytes() const { return dense && centers ? numel(ndim, bshape) * (int64_t)es : 0; }
+
+  // device bounds of slab rows [j0, j1) of the slab dim, and their strides (on stream st, after the slab's upload)
+  int slab(int64_t j0, int64_t j1, const SlabBufs& b, cudaStream_t st, const void** th, int64_t* strides) const {
+    if (!dense) {
+      for (int d = 0; d < ndim; ++d) strides[d] = bstrides[d];
+      *th = static_cast<const char*>(d_bcast) + (sd >= 0 ? (size_t)(j0 * bstrides[sd]) * es : 0);
+      return XG_OK;
+    }
+    int64_t ts[XG_MAX_NDIM], bs[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) {
+      ts[d] = tshape[d];
+      bs[d] = bshape[d];
+    }
+    if (sd >= 0) ts[sd] = bs[sd] = j1 - j0;
+    dense_strides(ndim, bs, strides);  // a slab's own dense layout, not the host strides
+    if (!centers) {
+      *th = b.in2;
+      return XG_OK;
+    }
+    *th = b.scratch;
+    return xg_stencil2(XG_OP_INTERP, dtype, b.in2, b.scratch, ndim, ts, axis, 1, 1, XG_BC_EXTEND, 0.0, nullptr,
+                       nullptr, nullptr, nullptr, nullptr, nullptr, st);
+  }
+};
+
+// Argument checks on theta that need no device: its extent along the axis, and (at centres) a layout the
+// center -> outer stencil can read.
+int check_theta(const char* fn, int ndim, const int64_t* tshape, const int64_t* strides, int axis, int centers) {
+  for (int d = 0; d < ndim; ++d)
+    if (strides[d] < 0) return xg_fail(XG_EINVAL, std::string(fn) + ": negative theta stride");
+  if (tshape[axis] > 1 && strides[axis] == 0)
+    return xg_fail(XG_EINVAL, std::string(fn) + ": theta must hold " + std::to_string(tshape[axis]) +
+                                  (centers ? " cell-centre values" : " cell bounds") +
+                                  " along the axis; it is broadcast along it");
+  if (centers && !theta_is_dense(ndim, tshape, strides)) {
+    int64_t cshape[XG_MAX_NDIM], cs[XG_MAX_NDIM];
+    compact_shape(ndim, tshape, strides, cshape);
+    dense_strides(ndim, cshape, cs);
+    for (int d = 0; d < ndim; ++d)
+      if (cshape[d] > 1 && strides[d] != cs[d])
+        return xg_fail(XG_EINVAL, std::string(fn) +
+                                      ": theta at cell centres must be C-contiguous in the dims it is not broadcast over");
+  }
+  return XG_OK;
+}
+
+// Build the plan once the session is open; theta holds `tn` values along the axis (n + 1 bounds, n centres, or the
+// n levels of the linear twin).  A broadcast theta goes up whole into aux slot 0; plan_theta_bounds makes the bounds
+// of one that holds centres.
+int plan_theta(PipeWorkspace* w, ThetaPlan* p, int dtype, const void* theta, const int64_t* strides, int centers,
+               int64_t tn, int ndim, const int64_t* shape, int axis) {
+  p->dtype = dtype;
+  p->es = dtype == XG_F32 ? 4 : 8;
+  p->ndim = ndim;
+  p->axis = axis;
+  p->centers = centers != 0;
+  for (int d = 0; d < ndim; ++d) p->tshape[d] = p->bshape[d] = shape[d];
+  p->tshape[axis] = tn;
+  p->bshape[axis] = p->centers ? tn + 1 : tn;
+  p->dense = theta_is_dense(ndim, p->tshape, strides);
+  if (p->dense) return XG_OK;
+  int rc = upload_aux(w, 0, theta, operand_span(strides, p->tshape, ndim, p->es), &p->d_bcast);
+  if (rc) return rc;
+  for (int d = 0; d < ndim; ++d) p->bstrides[d] = strides[d];
+  return XG_OK;
+}
+
+// the bounds of a broadcast theta held at centres, once, into aux slot 1, on the kernel stream (after aux_fence)
+int plan_theta_bounds(PipeWorkspace* w, ThetaPlan* p, const int64_t* strides) {
+  if (p->dense || !p->centers) return XG_OK;
+  int64_t cshape[XG_MAX_NDIM], cb[XG_MAX_NDIM];
+  compact_shape(p->ndim, p->tshape, strides, cshape);
+  for (int d = 0; d < p->ndim; ++d) cb[d] = cshape[d];
+  cb[p->axis] = p->bshape[p->axis];
+  int rc = ensure(&w->d_aux[1], &w->aux_cap[1], (size_t)numel(p->ndim, cb) * p->es);
+  if (rc) return rc;
+  rc = xg_stencil2(XG_OP_INTERP, p->dtype, p->d_bcast, w->d_aux[1], p->ndim, cshape, p->axis, 1, 1, XG_BC_EXTEND,
+                   0.0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, w->s_k);
+  if (rc) return rc;
+  dense_strides(p->ndim, cb, p->bstrides);
+  for (int d = 0; d < p->ndim; ++d)
+    if (cb[d] == 1) p->bstrides[d] = 0;  // broadcast again over phi's extent
+  p->d_bcast = w->d_aux[1];
+  return XG_OK;
+}
+
+// [C][L][R] views of phi, streamed theta and the result (shape-without-axis + trailing `m_out`) around the slab
+// dim of a transform twin, and the PipeExtra that streams theta and sizes the slabs
+struct TransformViews {
+  int sd = -1;
+  View3 vin{1, 1, 1}, vout{1, 1, 1};
+  PipeExtra ex;
+};
+
+TransformViews transform_views(int ndim, const int64_t* shape, int axis, int64_t m_out, const ThetaPlan& p,
+                               const void* theta) {
+  TransformViews t;
+  const int64_t es = (int64_t)p.es;
+  int64_t out_shape[XG_MAX_NDIM + 1];
+  int nd_o = 0;
+  for (int d = 0; d < ndim; ++d)
+    if (d != axis) out_shape[nd_o++] = shape[d];
+  out_shape[nd_o++] = m_out;
+  const int64_t out_bytes = numel(nd_o, out_shape) * es;
+  const int64_t total = numel(ndim, shape) * es + p.stream_bytes() + p.scratch_bytes() + out_bytes;
+  t.sd = transform_slab_dim(ndim, shape, axis, total);
+  const int64_t L = t.sd >= 0 ? shape[t.sd] : 1;
+  if (t.sd >= 0) {
+    t.vin = view3(ndim, shape, t.sd);
+    t.vout = view3(nd_o, out_shape, t.sd < axis ? t.sd : t.sd - 1);
+    t.ex.in2 = view3(ndim, p.tshape, t.sd);
+  } else {
+    t.vin = View3{1, 1, numel(ndim, shape)};
+    t.vout = View3{1, 1, out_bytes / es};
+    t.ex.in2 = View3{1, 1, numel(ndim, p.tshape)};
+  }
+  if (p.dense) t.ex.hin2 = theta;
+  t.ex.scratch_row_bytes = (size_t)(p.scratch_bytes() / L);
+  t.ex.row_bytes = total / L;
+  return t;
+}
+
 }  // namespace
 
 void xg_host_pipe_release() {
@@ -236,6 +458,12 @@ void xg_host_pipe_release() {
       if (w->d_in[i]) cudaFree(w->d_in[i]);
       w->d_in[i] = nullptr;
       w->in_cap[i] = 0;
+      if (w->d_in2[i]) cudaFree(w->d_in2[i]);
+      w->d_in2[i] = nullptr;
+      w->in2_cap[i] = 0;
+      if (w->d_scr[i]) cudaFree(w->d_scr[i]);
+      w->d_scr[i] = nullptr;
+      w->scr_cap[i] = 0;
       for (int k = 0; k < kMaxOut; ++k) {
         if (w->d_out[i][k]) cudaFree(w->d_out[i][k]);
         w->d_out[i][k] = nullptr;
@@ -313,12 +541,11 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
     rc = aux_fence(w);
     if (rc) return rc;
   }
-  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, void* d_in, void* const* d_out,
-                    cudaStream_t st) -> int {
+  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
     int64_t sshape[XG_MAX_NDIM];
     for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
     for (int k = 0; k < nout; ++k) {
-      const char* src = static_cast<const char*>(d_in);
+      const char* src = static_cast<const char*>(b.in);
       int slo = lo[k], shi = hi[k], sbc = bc[k];
       const void* hl = nullptr;
       const void* hh = nullptr;
@@ -340,7 +567,7 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
         src += (size_t)(j0 - i0) * vin.R * es;
         sshape[0] = j1 - j0;
       }
-      const int rc2 = xg_stencil2(op[k], dtype, src, d_out[k], ndim, sshape, axis[k], slo, shi, sbc, fill_value[k],
+      const int rc2 = xg_stencil2(op[k], dtype, src, b.out[k], ndim, sshape, axis[k], slo, shi, sbc, fill_value[k],
                                   nullptr, nullptr, nullptr, nullptr, hl, hh, st);
       if (rc2) return rc2;
     }
@@ -382,15 +609,15 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
   if (sd < 0) {  // 1-D: one slab = the whole line
     const View3 v{1, 1, shape[0]}, vo{1, 1, out_shape[0]};
     void* outs[1] = {out};
-    auto launch = [&](int64_t, int64_t, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
-      return xg_cumscan(dtype, d_in, d_out[0], ndim, shape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, d_pre,
+    auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      return xg_cumscan(dtype, b.in, b.out[0], ndim, shape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, d_pre,
                         pre_strides, d_post, post_strides, skipna, st);
     };
     return run_pipe(w, es, in, v, 1, outs, &vo, 0, launch);
   }
   const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
   void* outs[1] = {out};
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
+  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
     int64_t sshape[XG_MAX_NDIM];
     for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
     sshape[sd] = j1 - j0;
@@ -398,7 +625,7 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
     const char* qm = static_cast<const char*>(d_post);
     if (pm) pm += (size_t)(j0 * pre_strides[sd]) * es;
     if (qm) qm += (size_t)(j0 * post_strides[sd]) * es;
-    return xg_cumscan(dtype, d_in, d_out[0], ndim, sshape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, pm,
+    return xg_cumscan(dtype, b.in, b.out[0], ndim, sshape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, pm,
                       pre_strides, qm, post_strides, skipna, st);
   };
   return run_pipe(w, es, in, vin, 1, outs, &vout, 0, launch);
@@ -426,8 +653,8 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
   void* outs[1] = {out};
   if (sd < 0) {
     const View3 v{1, 1, shape[0]}, vo{1, 1, 1};
-    auto launch = [&](int64_t, int64_t, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
-      return xg_wreduce(dtype, d_in, d_w, w_strides, d_out[0], ndim, shape, axis, mode, skipna, st);
+    auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      return xg_wreduce(dtype, b.in, d_w, w_strides, b.out[0], ndim, shape, axis, mode, skipna, st);
     };
     return run_pipe(w, es, in, v, 1, outs, &vo, 0, launch);
   }
@@ -440,13 +667,13 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
     out_shape[nd_o++] = shape[d];
   }
   const View3 vin = view3(ndim, shape, sd), vout = view3(nd_o, out_shape, sd_o);
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
+  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
     int64_t sshape[XG_MAX_NDIM];
     for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
     sshape[sd] = j1 - j0;
     const char* wm = static_cast<const char*>(d_w);
     if (wm) wm += (size_t)(j0 * w_strides[sd]) * es;
-    return xg_wreduce(dtype, d_in, wm, w_strides, d_out[0], ndim, sshape, axis, mode, skipna, st);
+    return xg_wreduce(dtype, b.in, wm, w_strides, b.out[0], ndim, sshape, axis, mode, skipna, st);
   };
   return run_pipe(w, es, in, vin, 1, outs, &vout, 0, launch);
 }
@@ -468,12 +695,11 @@ extern "C" int xg_vinterp_linear_host(int dtype, const void* phi, const void* th
   int rc = ss.open(device);
   if (rc) return rc;
   PipeWorkspace* w = ss.w;
-  // theta (shared coordinate or a whole field) and target are uploaded whole: the field case costs one extra
-  // resident copy of theta, it is not the streamed operand
-  const void* d_theta = nullptr;
-  const void* d_target = nullptr;
-  rc = upload_aux(w, 0, theta, operand_span(theta_strides, shape, ndim, es), &d_theta);
+  // theta: a dense field streams beside phi, a broadcast one is uploaded whole (aux 0); target whole (aux 1)
+  ThetaPlan tp;
+  rc = plan_theta(w, &tp, dtype, theta, theta_strides, 0, shape[axis], ndim, shape, axis);
   if (rc) return rc;
+  const void* d_target = nullptr;
   int64_t tshape[XG_MAX_NDIM];
   for (int d = 0; d < ndim; ++d) tshape[d] = shape[d];
   tshape[axis] = m;
@@ -482,35 +708,108 @@ extern "C" int xg_vinterp_linear_host(int dtype, const void* phi, const void* th
   if (rc) return rc;
   rc = aux_fence(w);
   if (rc) return rc;
-  const int sd = first_free_dim(ndim, axis);
+  const TransformViews tv = transform_views(ndim, shape, axis, m, tp, theta);
+  tp.sd = tv.sd;
   void* outs[1] = {out};
-  if (sd < 0) {
-    const View3 v{1, 1, shape[0]}, vo{1, 1, m};
-    auto launch = [&](int64_t, int64_t, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
-      return xg_vinterp_linear(dtype, d_in, d_theta, theta_strides, d_target, target_strides, m, d_out[0], ndim, shape,
-                               axis, mask_edges, bypass_checks, logarithmic, st);
-    };
-    return run_pipe(w, es, phi, v, 1, outs, &vo, 0, launch);
-  }
-  // result shape = shape without `axis`, then m appended last
-  int64_t out_shape[XG_MAX_NDIM + 1];
-  int nd_o = 0, sd_o = 0;
-  for (int d = 0; d < ndim; ++d) {
-    if (d == axis) continue;
-    if (d == sd) sd_o = nd_o;
-    out_shape[nd_o++] = shape[d];
-  }
-  out_shape[nd_o++] = m;
-  const View3 vin = view3(ndim, shape, sd), vout = view3(nd_o, out_shape, sd_o);
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, void* d_in, void* const* d_out, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM];
+  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+    int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
     for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    sshape[sd] = j1 - j0;
-    const char* th = static_cast<const char*>(d_theta) + (size_t)(j0 * theta_strides[sd]) * es;
     const char* tg = static_cast<const char*>(d_target);
-    if (target_strides) tg += (size_t)(j0 * target_strides[sd]) * es;
-    return xg_vinterp_linear(dtype, d_in, th, theta_strides, tg, target_strides, m, d_out[0], ndim, sshape, axis,
+    if (tv.sd >= 0) {
+      sshape[tv.sd] = j1 - j0;
+      if (target_strides) tg += (size_t)(j0 * target_strides[tv.sd]) * es;
+    }
+    const void* th = nullptr;
+    const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
+    if (rc2) return rc2;
+    return xg_vinterp_linear(dtype, b.in, th, th_strides, tg, target_strides, m, b.out[0], ndim, sshape, axis,
                              mask_edges, bypass_checks, logarithmic, st);
   };
-  return run_pipe(w, es, phi, vin, 1, outs, &vout, 0, launch);
+  return run_pipe(w, es, phi, tv.vin, 1, outs, &tv.vout, 0, launch, tv.ex);
+}
+
+// ---------------------------------------------------------------------------------------------------
+extern "C" int xg_vinterp_conservative_host(int dtype, const void* phi, const void* theta,
+                                            const int64_t* theta_strides, int theta_at_centers,
+                                            const void* target_bins, int64_t m, int flip_out, void* out, int ndim,
+                                            const int64_t* shape, int axis, int device) {
+  if (!phi || !theta || !target_bins || !out || !shape)
+    return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: null pointer");
+  if (!theta_strides) return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: theta strides missing");
+  if (dtype != XG_F32 && dtype != XG_F64)
+    return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: dtype must be XG_F32 or XG_F64");
+  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: bad ndim");
+  if (axis < 0 || axis >= ndim) return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: axis out of range");
+  for (int d = 0; d < ndim; ++d)
+    if (shape[d] < 0) return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: negative extent");
+  if (m < 2) return xg_fail(XG_EINVAL, "xg_vinterp_conservative_host: need at least two bin edges");
+  const int64_t n = shape[axis];
+  int64_t tshape[XG_MAX_NDIM];
+  for (int d = 0; d < ndim; ++d) tshape[d] = shape[d];
+  tshape[axis] = theta_at_centers ? n : n + 1;
+  int rc = check_theta("xg_vinterp_conservative_host", ndim, tshape, theta_strides, axis, theta_at_centers);
+  if (rc) return rc;
+  const size_t es = dtype == XG_F32 ? 4 : 8;
+  int64_t ncols = 1;
+  for (int d = 0; d < ndim; ++d)
+    if (d != axis) ncols *= shape[d];
+  if (ncols == 0) return XG_OK;
+  if (n == 0) {  // no source cells: every bin receives nothing and stays NaN, as in k_vconserv
+    const int64_t count = ncols * (m - 1);
+    if (dtype == XG_F32)
+      for (int64_t i = 0; i < count; ++i) static_cast<float*>(out)[i] = NAN;
+    else
+      for (int64_t i = 0; i < count; ++i) static_cast<double*>(out)[i] = NAN;
+    return XG_OK;
+  }
+  Session ss;
+  rc = ss.open(device);
+  if (rc) return rc;
+  PipeWorkspace* w = ss.w;
+  // theta: streamed (dense) or whole in aux 0 (its bounds in aux 1 at centres); bins whole in aux 2
+  ThetaPlan tp;
+  rc = plan_theta(w, &tp, dtype, theta, theta_strides, theta_at_centers, tshape[axis], ndim, shape, axis);
+  if (rc) return rc;
+  const void* d_bins = nullptr;
+  rc = upload_aux(w, 2, target_bins, (size_t)m * es, &d_bins);
+  if (rc) return rc;
+  rc = aux_fence(w);
+  if (rc) return rc;
+  rc = plan_theta_bounds(w, &tp, theta_strides);
+  if (rc) return rc;
+  const TransformViews tv = transform_views(ndim, shape, axis, m - 1, tp, theta);
+  tp.sd = tv.sd;
+  void* outs[1] = {out};
+  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+    int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+    if (tv.sd >= 0) sshape[tv.sd] = j1 - j0;
+    const void* th = nullptr;
+    const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
+    if (rc2) return rc2;
+    return xg_vinterp_conservative(dtype, b.in, th, th_strides, d_bins, m, flip_out, b.out[0], ndim, sshape, axis,
+                                   st);
+  };
+  return run_pipe(w, es, phi, tv.vin, 1, outs, &tv.vout, 0, launch, tv.ex);
+}
+
+extern "C" int xg_host_pipe_workspace_bytes(int device, int64_t* bytes) {
+  if (!bytes) return xg_fail(XG_EINVAL, "xg_host_pipe_workspace_bytes: null pointer");
+  *bytes = 0;
+  PipeWorkspace* w = nullptr;
+  {
+    std::lock_guard<std::mutex> reg(g_reg_mutex);
+    for (PipeWorkspace* x : g_pipes)
+      if (x->device == device) w = x;
+  }
+  if (!w) return XG_OK;
+  std::lock_guard<std::mutex> lock(w->mu);
+  size_t total = 0;
+  for (int i = 0; i < kSlots; ++i) {
+    total += w->in_cap[i] + w->in2_cap[i] + w->scr_cap[i];
+    for (int k = 0; k < kMaxOut; ++k) total += w->out_cap[i][k];
+  }
+  for (int i = 0; i < kMaxAux; ++i) total += w->aux_cap[i];
+  *bytes = (int64_t)total;
+  return XG_OK;
 }

@@ -923,3 +923,45 @@ def vinterp_linear_host(phi: np.ndarray, theta: np.ndarray, target: np.ndarray, 
             int(bool(bypass_checks)), int(bool(logarithmic)), dev)
         _capi.check(rc)
     return out
+
+
+def vinterp_conservative_host(phi: np.ndarray, theta: np.ndarray, target_bins: np.ndarray, axis: int,
+                              theta_at_centers: bool = False, device: Optional[int] = None) -> np.ndarray:
+    """Host twin of :func:`vinterp_conservative` (``xg_vinterp_conservative_host``): slabs of ``phi`` (and of
+    ``theta`` when it is a full field) stream through the GPU.  With ``theta_at_centers``, ``theta`` holds n
+    cell-centre values along ``axis`` and its bounds are those of ``grid.interp(theta, axis, padding="extend")``."""
+    lib = _capi.load()
+    phi = _host_field(phi, "phi")
+    theta = np.asarray(theta)
+    target_bins = np.asarray(target_bins)
+    if not (phi.dtype == theta.dtype == target_bins.dtype == np.float32):
+        phi, theta, target_bins = (phi.astype(np.float64, copy=False), theta.astype(np.float64, copy=False),
+                                   target_bins.astype(np.float64, copy=False))
+    if target_bins.ndim != 1:
+        raise ValueError("target bins must be 1-D")
+    phi = np.ascontiguousarray(phi)
+    axis = _norm_axis(axis, phi.ndim)
+    shape = list(phi.shape)
+    tshape = list(shape)
+    tshape[axis] = shape[axis] + (0 if theta_at_centers else 1)
+    if theta.ndim == phi.ndim and theta.shape[axis] != tshape[axis]:
+        what = "cell-centre values" if theta_at_centers else "cell bounds"
+        raise ValueError(f"theta needs {tshape[axis]} {what} along the axis, got {theta.shape[axis]}")
+    diffs = target_bins[1:] - target_bins[:-1]
+    if bool((diffs < 0).all()):  # transform.py:167-176
+        flip, bins = 1, np.ascontiguousarray(target_bins[::-1])
+    elif bool((diffs > 0).all()):
+        flip, bins = 0, np.ascontiguousarray(target_bins)
+    else:
+        raise ValueError("Target values are not monotonic")
+    kt, th_ptr, th_st = _host_operand(theta, tshape, phi.dtype, "theta")
+    m = int(bins.size)
+    out_shape = [s for d, s in enumerate(shape) if d != axis] + [m - 1]
+    out = pinned_empty(out_shape, phi.dtype)
+    dev = torch.cuda.current_device() if device is None else int(device)
+    if out.size:
+        rc = lib.xg_vinterp_conservative_host(
+            _capi.dtype_code(phi.dtype), phi.ctypes.data, th_ptr, th_st, int(bool(theta_at_centers)),
+            bins.ctypes.data, m, flip, out.ctypes.data, phi.ndim, _capi.i64_array(shape), axis, dev)
+        _capi.check(rc)
+    return out

@@ -138,10 +138,19 @@ def linear_interpolation(phi, theta, target_theta_levels, phi_dim, theta_dim, ta
 
 def interp_1d_conservative(phi, theta, target_theta_bins):
     """Array-level entry point with the reference's signature (transform.py:145-191):
-    ``phi[..., n], theta[..., n+1], bins[m] -> [..., m-1]`` along the LAST axis."""
+    ``phi[..., n], theta[..., n+1], bins[m] -> [..., m-1]`` along the LAST axis.
+    numpy in -> numpy out (slabs streamed through the GPU); CUDA tensors stay on the device."""
     from . import ops
     from .device import as_device_tensor, result_like
+    from .labeled import is_device_array
 
+    if not any(is_device_array(a) for a in (phi, theta, target_theta_bins)) and _cuda_device() is not None:
+        p, th, tb = np.asarray(phi), np.asarray(theta), np.asarray(target_theta_bins)
+        if p.shape[-1] != th.shape[-1] - 1:
+            raise AssertionError("phi needs one value per cell: phi.shape[-1] == theta.shape[-1] - 1")
+        if tb.ndim != 1:
+            raise AssertionError("target_theta_bins must be 1-D")
+        return ops.vinterp_conservative_host(p, th, tb, -1)
     p, host = as_device_tensor(phi)
     th, _ = as_device_tensor(theta, p.device)
     tb, _ = as_device_tensor(target_theta_bins, p.device)
@@ -154,10 +163,39 @@ def interp_1d_conservative(phi, theta, target_theta_bins):
     return result_like(ops.vinterp_conservative(p, th, tb, -1), host)
 
 
+def _cuda_device(phi=None, grid=None):
+    """The CUDA device a call on ``phi`` runs on, or None without one (the device route then raises its own error)."""
+    from . import device as _device
+
+    try:
+        dev = grid._device_for(phi) if grid is not None else _device.default_device()
+    except RuntimeError:
+        return None
+    return dev if dev.type == "cuda" else None
+
+
+def _conservative_host_device(phi, theta, target_theta_levels, grid):
+    """The CUDA device through which ``xg_vinterp_conservative_host`` streams a numpy-backed remap, or None when
+    the device route applies: device or mixed inputs, a field that is not f32 / f64, no CUDA device."""
+    if (phi.is_device or theta.is_device or target_theta_levels.is_device
+            or np.asarray(phi.data).dtype not in (np.float32, np.float64)):
+        return None
+    return _cuda_device(phi, grid)
+
+
 def conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_dim, target_dim,
                                suffix="", grid=None):
     """Labelled wrapper (transform.py:252-276): bins along ``target_dim`` (one fewer than the
     levels), coordinate = bin centres."""
+    return _conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_dim, target_dim, suffix,
+                                       grid)
+
+
+def _conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_dim, target_dim, suffix="",
+                                grid=None, theta_at_centers=False):
+    """:func:`conservative_interpolation`; with ``theta_at_centers`` (numpy inputs only) ``theta`` holds the n cell
+    centres along ``theta_dim`` and the remap uses the bounds ``grid.interp(theta, axis, padding="extend")`` gives,
+    made slab by slab on the device."""
     from . import ops
     from .device import as_device_tensor, result_like
 
@@ -167,9 +205,32 @@ def conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_d
         raise NotImplementedError(
             "Conservative transformation is not yet supported for multi-dimensional targets."
         )
+    host_dev = _conservative_host_device(phi, theta, target_theta_levels, grid)
+    if theta_at_centers and host_dev is None:
+        raise ValueError("theta at cell centres is taken by the host route only (numpy inputs, a CUDA device)")
+    extra = [d for d in theta.dims if d not in phi.dims and d != theta_dim]
+    if host_dev is not None:
+        # numpy-backed fields: slabs of phi (and of a full theta field) stream through the GPU
+        # (xg_vinterp_conservative_host: H2D || kernel || D2H) instead of one upload + one download
+        if extra:
+            raise ValueError(f"target data has dimensions {extra} that the data does not have")
+        th_dims = [d if d != theta_dim else phi_dim for d in theta.dims]
+        th = np.asarray(theta.values)
+        present = [d for d in phi.dims if d in th_dims]
+        perm = [th_dims.index(d) for d in present]
+        if perm != list(range(len(perm))):
+            th = np.transpose(th, perm)
+        sizes = dict(zip(th_dims, theta.shape))
+        need = phi.sizes[phi_dim] + (0 if theta_at_centers else 1)
+        if sizes[phi_dim] != need:
+            what = "cell-centre values" if theta_at_centers else "cell bounds"
+            raise ValueError(f"`target_data` needs {need} {what} along {theta_dim!r}, got {sizes[phi_dim]}")
+        th = th.reshape([sizes[d] if d in th_dims else 1 for d in phi.dims])
+        out = ops.vinterp_conservative_host(np.asarray(phi.data), th, np.asarray(target_theta_levels.values),
+                                            phi.get_axis_num(phi_dim), theta_at_centers, device=host_dev.index)
+        return _conservative_result(out, phi, phi_dim, target_theta_levels, target_dim, suffix)
     device = grid._device_for(phi) if grid is not None else None
     x, host = as_device_tensor(phi.data, device)
-    extra = [d for d in theta.dims if d not in phi.dims and d != theta_dim]
     if extra:
         raise ValueError(f"target data has dimensions {extra} that the data does not have")
     axis_num = phi.get_axis_num(phi_dim)
@@ -187,15 +248,31 @@ def conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_d
     th_t = th_t.reshape([sizes[d] if d in th_dims else 1 for d in phi.dims])
     tg_t, _ = as_device_tensor(target_theta_levels.data, x.device)
     out = ops.vinterp_conservative(x, th_t, tg_t, axis_num)
+    return _conservative_result(result_like(out, host), phi, phi_dim, target_theta_levels, target_dim, suffix)
+
+
+def _conservative_result(out, phi, phi_dim, target_theta_levels, target_dim, suffix):
     out_dims = tuple(d for d in phi.dims if d != phi_dim) + (target_dim,)
     coords = {k: c for k, c in phi.coords.items()
               if phi_dim not in c.dims and k != target_dim and all(d in out_dims for d in c.dims)}
     levels = target_theta_levels.values
     coords[target_dim] = ((target_dim,), (levels[1:] + levels[:-1]) / 2)  # transform.py:270-272
-    res = DataArray(result_like(out, host), dims=out_dims, coords=coords)
+    res = DataArray(out, dims=out_dims, coords=coords)
     if phi.name:
         res.name = phi.name + suffix
     return res
+
+
+def _fuse_centre_bounds(phi, theta, target, grid):
+    """Whether the remap of numpy fields may make theta's bounds itself: the host route applies, and theta's dtype
+    is the remap's, so the center -> outer interp rounds as grid.interp's would (grid.interp works in theta's own
+    dtype, integers in f64; the remap works in f32 only when phi, theta and the bins all are f32)."""
+    if _conservative_host_device(phi, theta, target, grid) is None:
+        return False
+    th_dt = np.asarray(theta.data).dtype
+    th_dt = th_dt if th_dt in (np.float32, np.float64) else np.dtype(np.float64)
+    all_f32 = np.asarray(phi.data).dtype == th_dt == np.asarray(target.data).dtype == np.float32
+    return th_dt == (np.float32 if all_f32 else np.float64)
 
 
 def transform(grid, axis_name, da, target, target_data=None, target_dim=None, method="linear",
@@ -291,6 +368,13 @@ def transform(grid, axis_name, da, target, target_data=None, target_dim=None, me
                 "The `target data` input is not located on the cell bounds. This method will continue with linear interpolation with repeated boundary values. For most accurate results provide values on cell bounds.",
                 UserWarning,
             )
+            center = axis.coords.get("center")
+            if (center is not None and center in target_data.dims and axis.default_shifts.get("center") == "outer"
+                    and target_data.sizes[center] == da.sizes[dim] and _fuse_centre_bounds(da, target_data, target, grid)):
+                # numpy fields: the n + 1 bounds grid.interp would give are made slab by slab on the device, beside
+                # the remap, instead of a round trip of the bounds through host memory
+                return _conservative_interpolation(da, target_data, target, dim, center, target_dim, grid=grid,
+                                                   theta_at_centers=True)
             target_data = grid.interp(target_data, axis_name, padding="extend")
         return conservative_interpolation(da, target_data, target, dim, target_data_dim, target_dim, grid=grid)
     raise ValueError(f"unknown transform method {method!r}")
