@@ -381,8 +381,9 @@ XG_API int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, vo
                                      const void* post, const int64_t* post_strides, int seam_axis, int skip,
                                      int64_t mirror, int64_t period, int negate, int device);
 
-/* Device bytes the workspace of xg_stencil2_host, xg_stencil_pair_host and their variants holds on `device`
- * (slot buffers, metrics, halo planes); 0 before the first call or after xg_host_workspace_release. */
+/* Device bytes the one workspace of the *_host entry points holds on `device` (slot buffers, halo planes,
+ * scratch, whole-call operands such as metrics); 0 before the first call or after xg_host_workspace_release.
+ * Same number as xg_host_pipe_workspace_bytes. */
 XG_API int xg_host_workspace_bytes(int device, int64_t* bytes);
 
 /*
@@ -433,12 +434,12 @@ XG_API int xg_vinterp_conservative_host(int dtype, const void* phi, const void* 
                                  const void* target_bins, int64_t m, int flip_out, void* out, int ndim,
                                  const int64_t* shape, int axis, int device);
 
-/* Device bytes the workspace of xg_stencil2_host_multi, xg_cumscan_host, xg_wreduce_host and the two transform twins
- * holds on `device` (slot buffers, theta-bounds scratch, aux operands); 0 before the first call or after
- * xg_host_workspace_release. */
+/* Device bytes the one workspace of the *_host entry points holds on `device`: the same number as
+ * xg_host_workspace_bytes, kept for callers of the multi, scan, reduce and transform twins. */
 XG_API int xg_host_pipe_workspace_bytes(int device, int64_t* bytes);
 
-/* Free the cached device slabs / streams of the *_host entry points. */
+/* Free the cached device buffers of the *_host entry points (waiting for a call in progress on a device to
+ * finish first); their streams and events are kept for later calls. */
 XG_API int xg_host_workspace_release(void);
 
 #ifdef __cplusplus

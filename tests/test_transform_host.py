@@ -85,7 +85,7 @@ def slab_dim(shape, axis, per_index_total_bytes, budget=128 << 20):
 
 
 def slab_rows(L, row_bytes, budget=128 << 20):
-    """xg_host_pipe.cu slab_rows: the budget's rows, at least one, and at least 4 slabs when the dim allows."""
+    """xg_host.cu slab_rows: the budget's rows, at least one, and at least 4 slabs when the dim allows."""
     rows = max(1, budget // row_bytes) if row_bytes > 0 else L
     return max(1, min(rows, (L + 3) // 4))
 

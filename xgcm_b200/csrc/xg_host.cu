@@ -1,55 +1,39 @@
-// xg_stencil2_host — the fused stencil on HOST buffers, streamed through the GPU.
+// The host-buffer entry points' slab engine, and the stencil / pair entry points on it.
 //
-// This is the call the reference-facing API makes for numpy-backed fields: the
-// whole of xgcm/padding.py:575-616 + gridops.py + the metric passes for one axis,
-// with host<->device copies inside.  The field is cut into slabs along dim 0
-// (contiguous in host memory).  Three streams form a pipeline
-//     H2D(slab s+1)  ||  kernel(slab s)  ||  D2H(slab s-1)
-// so PCIe runs full duplex and the kernel time hides entirely behind the copies.
-// When dim 0 is the operated axis the slabs overlap by the one-cell halo and the
-// exterior halo plane (periodic wrap) is uploaded once.
+// Numpy-backed fields are cut into slabs along one dimension and streamed through the GPU.  Three streams form a
+// pipeline
+//     H2D(slab s+1)  ||  kernel(s)(slab s)  ||  D2H(slab s-1)
+// over three slots, so PCIe runs full duplex and the kernel time hides behind the copies.  Session::run is that
+// pipeline for every host entry point (this file and xg_host_pipe.cu): it takes a [C][L][R] view of the input
+// around the slab dim (strided 2-D copies when C > 1) and a launch callback that runs a slab's kernels.  A slab of
+// result rows [j0, j1) reads input rows [j0 - lo_rows, j1 + hi_rows); rows the previous slab already holds are
+// copied device-to-device, so each input row crosses PCIe once.
 //
-// xg_stencil2_host_fold / xg_stencil2_host_connected run the same slab loop with a per-slab halo stage
-// on the kernel stream: the slab's halo_lo / halo_hi planes are built from the slab buffers (one
-// xg_fold_rows launch, or the face-connection copy list clipped to the slab and replayed with
-// xg_strided_copy_batch) just before its xg_stencil2 launch.  Dim 0 is then a batch dim, so the planes
-// of one slab depend on that slab (and the partner component's slab) alone.
+// One Workspace per device holds the streams, the events and three classes of buffers: per slot, what the copy
+// streams touch (the input slab, a second streamed input, up to kMaxOut result slabs); once, what only the kernel
+// stream touches (the per-slab halo planes, a scratch buffer); and the aux operands uploaded whole once per call.
+// Its mutex makes calls on one device take turns (they would fight for PCIe anyway); calls on different devices
+// run concurrently.  Streams and events live for the process; xg_host_workspace_release() frees the buffers.
 //
-// xg_stencil_pair_host / xg_stencil_pair_host_fold run the two-field composite on the same loop: field a
-// is the slab input, field b streams through the partner slots, and each slab is one xg_stencil_pair_halo
-// launch (after the xg_fold_rows launch of b's folded row, for the fold).
-//
-// Workspace (device slabs + events + streams) is cached per device and reused;
-// xg_host_workspace_release() frees it.
+// The stencil entry points here slab dim 0.  xg_stencil2_host: when dim 0 is the operated axis, consecutive slabs
+// overlap by the one-cell halo and the exterior halo plane (periodic wrap) is uploaded once.
+// xg_stencil2_host_fold / xg_stencil2_host_connected: dim 0 is a batch dim, and a per-slab halo stage on the kernel
+// stream builds the slab's halo_lo / halo_hi planes from the slab buffers (one xg_fold_rows launch, or the
+// face-connection copy list clipped to the slab and replayed with xg_strided_copy_batch) just before its
+// xg_stencil2 launch.  xg_stencil_pair_host / xg_stencil_pair_host_fold: field a is the slab input, field b the
+// second streamed input, and each slab is one xg_stencil_pair_halo launch (after the xg_fold_rows launch of b's
+// folded row, for the fold).
 #include <stdlib.h>
 
-#include <mutex>
 #include <vector>
 
-#include "xg_common.cuh"
+#include "xg_host.cuh"
+
+namespace xg_host {
 
 namespace {
 
 constexpr int kSlots = 3;
-
-struct Workspace {
-  int device = -1;
-  std::mutex mu;  // one host call at a time per device; different devices run concurrently
-  size_t slab_in_bytes = 0, slab_out_bytes = 0, metric_bytes[3] = {0, 0, 0}, halo_bytes = 0;
-  size_t partner_bytes = 0, const_bytes = 0;
-  void* d_in[kSlots] = {nullptr, nullptr, nullptr};
-  void* d_out[kSlots] = {nullptr, nullptr, nullptr};
-  void* d_partner[kSlots] = {nullptr, nullptr, nullptr};  // second vector component, or field b of a pair
-  void* d_metric[3] = {nullptr, nullptr, nullptr};       // pre, post, and pre_a of a pair
-  void* d_halo[2] = {nullptr, nullptr};  // wrap planes along dim 0, or the per-slab lo / hi halo planes
-  void* d_const = nullptr;               // the fill constant the unconnected face edges copy from
-  cudaStream_t s_h2d = nullptr, s_k = nullptr, s_d2h = nullptr;
-  cudaEvent_t e_up[kSlots], e_done[kSlots], e_down[kSlots];
-  bool events = false;
-};
-
-std::mutex g_ws_mutex;
-std::vector<Workspace*> g_ws;
 
 #define XG_CUDA(call)                                                                   \
   do {                                                                                  \
@@ -58,40 +42,102 @@ std::vector<Workspace*> g_ws;
       return xg_fail(XG_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_));     \
   } while (0)
 
-int ensure(void** p, size_t* have, size_t want) {
-  if (*have >= want && *p) return XG_OK;
-  if (*p) XG_CUDA(cudaFree(*p));
-  *p = nullptr;
-  *have = 0;
-  if (want == 0) return XG_OK;
-  XG_CUDA(cudaMalloc(p, want));
-  *have = want;
-  return XG_OK;
-}
+}  // namespace
 
-int get_workspace(int device, Workspace** out) {
-  for (Workspace* w : g_ws)
-    if (w->device == device) {
-      *out = w;
-      return XG_OK;
+struct Workspace {
+  struct Buf {
+    void* p = nullptr;
+    size_t cap = 0;
+  };
+  int device = -1;
+  std::mutex mu;  // held by the call streaming through the workspace, and by release
+  cudaStream_t s_h2d = nullptr, s_k = nullptr, s_d2h = nullptr;
+  cudaEvent_t e_up[kSlots], e_done[kSlots], e_down[kSlots], e_aux;
+  bool ready = false;                                  // streams and events created
+  Buf in[kSlots], in2[kSlots], out[kSlots][kMaxOut];  // per slot: touched by the copy streams
+  Buf scratch, plane[2];                               // once: touched by the kernel stream alone
+  Buf aux[kNumAux];                                    // uploaded whole, once per call
+
+  template <class F>
+  void each_buf(F f) {
+    for (int i = 0; i < kSlots; ++i) {
+      f(in[i]);
+      f(in2[i]);
+      for (Buf& b : out[i]) f(b);
     }
-  Workspace* w = new Workspace();
-  w->device = device;
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_h2d, cudaStreamNonBlocking));
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_k, cudaStreamNonBlocking));
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_d2h, cudaStreamNonBlocking));
-  for (int i = 0; i < kSlots; ++i) {
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_up[i], cudaEventDisableTiming));
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_done[i], cudaEventDisableTiming));
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_down[i], cudaEventDisableTiming));
+    f(scratch);
+    f(plane[0]);
+    f(plane[1]);
+    for (Buf& b : aux) f(b);
   }
-  w->events = true;
-  g_ws.push_back(w);
-  *out = w;
+};
+
+namespace {
+
+std::mutex g_registry;          // guards g_ws
+std::vector<Workspace*> g_ws;  // one per device, kept for the process
+
+int ensure(Workspace::Buf& b, size_t want) {
+  if (b.cap >= want && b.p) return XG_OK;
+  if (b.p) XG_CUDA(cudaFree(b.p));
+  b = Workspace::Buf();
+  if (want == 0) return XG_OK;
+  XG_CUDA(cudaMalloc(&b.p, want));
+  b.cap = want;
   return XG_OK;
 }
 
-// bytes spanned by a broadcast operand laid out with `strides` over `shape`
+Workspace* find_workspace(int device) {  // caller holds g_registry
+  for (Workspace* w : g_ws)
+    if (w->device == device) return w;
+  return nullptr;
+}
+
+// `height` rows of `width` bytes, one cudaMemcpyAsync when there is one row
+int copy_rows(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, int64_t height,
+              cudaMemcpyKind kind, cudaStream_t st) {
+  if (width == 0 || height == 0) return XG_OK;
+  if (height == 1) XG_CUDA(cudaMemcpyAsync(dst, src, width, kind, st));
+  else XG_CUDA(cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, (size_t)height, kind, st));
+  return XG_OK;
+}
+
+// rows [r0, r1) of the slab dim of host array `host` (view v) <-> the device block at `dev`, whose C pieces hold
+// `dev_rows` rows each
+int copy_slab(void* dev, int64_t dev_rows, const void* host, const View3& v, int64_t r0, int64_t r1, size_t es,
+              bool to_device, cudaStream_t st) {
+  char* h = const_cast<char*>(static_cast<const char*>(host)) + (size_t)r0 * v.R * es;
+  const size_t width = (size_t)(r1 - r0) * v.R * es, hpitch = (size_t)v.L * v.R * es;
+  const size_t dpitch = (size_t)dev_rows * v.R * es;
+  if (to_device) return copy_rows(dev, dpitch, h, hpitch, width, v.C, cudaMemcpyHostToDevice, st);
+  return copy_rows(h, hpitch, dev, dpitch, width, v.C, cudaMemcpyDeviceToHost, st);
+}
+
+// rows per slab of a slab dim of extent L whose one row moves `row_bytes`
+int64_t slab_rows(int64_t L, int64_t row_bytes, bool edge_pairs) {
+  int64_t rows = row_bytes > 0 ? slab_budget_bytes() / row_bytes : L;
+  if (rows < 1) rows = 1;
+  if (rows > (L + 3) / 4) rows = (L + 3) / 4;  // at least 4 slabs when the dim allows: overlap
+  if (rows < 1) rows = 1;
+  if (edge_pairs) {
+    // e.g. an extrapolated halo is 2 A[edge] - A[next]: the slab that touches an edge must hold two input rows,
+    // i.e. no one-row slab at either end (a one-row tail is merged by growing the slab height)
+    if (rows < 2) rows = 2;
+    while (rows < L && L % rows == 1) ++rows;
+    if (rows > L) rows = L;
+  }
+  return rows;
+}
+
+}  // namespace
+
+View3 view3(int ndim, const int64_t* shape, int sd) {
+  View3 v{1, ndim ? shape[sd] : 1, 1};
+  for (int d = 0; d < sd; ++d) v.C *= shape[d];
+  for (int d = sd + 1; d < ndim; ++d) v.R *= shape[d];
+  return v;
+}
+
 size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size_t es) {
   int64_t last = 0;
   for (int d = 0; d < ndim; ++d)
@@ -99,41 +145,148 @@ size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size
   return (size_t)(last + 1) * es;
 }
 
-}  // namespace
-
-void xg_host_pipe_release();  // xg_host_pipe.cu
-
-extern "C" int xg_host_workspace_release(void) {
-  xg_host_pipe_release();
-  std::lock_guard<std::mutex> lock(g_ws_mutex);
-  for (Workspace* w : g_ws) {
-    cudaSetDevice(w->device);
-    for (int i = 0; i < kSlots; ++i) {
-      if (w->d_in[i]) cudaFree(w->d_in[i]);
-      if (w->d_out[i]) cudaFree(w->d_out[i]);
-      if (w->d_partner[i]) cudaFree(w->d_partner[i]);
-      if (w->events) {
-        cudaEventDestroy(w->e_up[i]);
-        cudaEventDestroy(w->e_done[i]);
-        cudaEventDestroy(w->e_down[i]);
-      }
-    }
-    for (int i = 0; i < 3; ++i)
-      if (w->d_metric[i]) cudaFree(w->d_metric[i]);
-    for (int i = 0; i < 2; ++i)
-      if (w->d_halo[i]) cudaFree(w->d_halo[i]);
-    if (w->d_const) cudaFree(w->d_const);
-    if (w->s_h2d) cudaStreamDestroy(w->s_h2d);
-    if (w->s_k) cudaStreamDestroy(w->s_k);
-    if (w->s_d2h) cudaStreamDestroy(w->s_d2h);
-    delete w;
+int64_t slab_budget_bytes() {
+  int64_t target_bytes = 128ll << 20;
+  if (const char* env = getenv("XG_HOST_SLAB_MB")) {  // tuning knob (benchmarks only)
+    const long mb = atol(env);
+    if (mb >= 1 && mb <= 4096) target_bytes = (int64_t)mb << 20;
   }
-  g_ws.clear();
+  return target_bytes;
+}
+
+Session::~Session() {
+  if (w_ && w_->ready)
+    for (cudaStream_t st : {w_->s_h2d, w_->s_k, w_->s_d2h}) cudaStreamSynchronize(st);
+}
+
+int Session::open(int device) {
+  XG_CUDA(cudaSetDevice(device));
+  {
+    std::lock_guard<std::mutex> reg(g_registry);
+    w_ = find_workspace(device);
+    if (!w_) {
+      w_ = new Workspace();
+      w_->device = device;
+      g_ws.push_back(w_);
+    }
+  }
+  lock_ = std::unique_lock<std::mutex>(w_->mu);
+  if (w_->ready) return XG_OK;
+  for (cudaStream_t* st : {&w_->s_h2d, &w_->s_k, &w_->s_d2h})
+    XG_CUDA(cudaStreamCreateWithFlags(st, cudaStreamNonBlocking));
+  for (int i = 0; i < kSlots; ++i)
+    for (cudaEvent_t* e : {&w_->e_up[i], &w_->e_done[i], &w_->e_down[i]})
+      XG_CUDA(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  XG_CUDA(cudaEventCreateWithFlags(&w_->e_aux, cudaEventDisableTiming));
+  w_->ready = true;
+  return XG_OK;
+}
+
+int Session::aux(Aux a, size_t bytes, void** dev) {
+  int rc = ensure(w_->aux[a], bytes);
+  if (rc) return rc;
+  *dev = w_->aux[a].p;
+  return XG_OK;
+}
+
+int Session::upload(Aux a, const void* host, size_t bytes, const void** dev) {
+  *dev = nullptr;
+  if (!host) return XG_OK;
+  void* d = nullptr;
+  int rc = aux(a, bytes, &d);
+  if (rc) return rc;
+  XG_CUDA(cudaMemcpyAsync(d, host, bytes, cudaMemcpyHostToDevice, w_->s_h2d));
+  *dev = d;
+  return XG_OK;
+}
+
+int Session::fence() {
+  XG_CUDA(cudaEventRecord(w_->e_aux, w_->s_h2d));
+  XG_CUDA(cudaStreamWaitEvent(w_->s_k, w_->e_aux, 0));
+  return XG_OK;
+}
+
+cudaStream_t Session::kernel_stream() const { return w_->s_k; }
+
+int Session::run(size_t es, const void* hin, const View3& in, int nout, void* const* hout, const View3* out,
+                 const LaunchFn& launch, const PipeExtra& ex) {
+  Workspace* w = w_;
+  const int64_t L = out[0].L;
+  if (in.L == 0 || in.C == 0 || in.R == 0 || L == 0) return XG_OK;
+  const int64_t rows = slab_rows(L, ex.row_bytes > 0 ? ex.row_bytes : in.C * in.R * (int64_t)es, ex.edge_pairs);
+  const int64_t nslab = xg_ceil_div(L, rows);
+  int rc = XG_OK;
+  for (int i = 0; rc == XG_OK && i < kSlots; ++i) {
+    rc = ensure(w->in[i], (size_t)(in.C * (rows + ex.lo_rows + ex.hi_rows) * in.R) * es);
+    if (rc == XG_OK && ex.hin2) rc = ensure(w->in2[i], (size_t)(ex.in2.C * rows * ex.in2.R) * es);
+    for (int k = 0; rc == XG_OK && k < nout; ++k)
+      rc = ensure(w->out[i][k], (size_t)(out[k].C * rows * out[k].R) * es);
+  }
+  if (rc == XG_OK) rc = ensure(w->scratch, ex.scratch_row_bytes * (size_t)rows);
+  for (int k = 0; rc == XG_OK && k < 2; ++k) rc = ensure(w->plane[k], ex.plane_row_bytes * (size_t)rows);
+  if (rc) return rc;
+
+  const size_t row = (size_t)in.R * es;  // bytes of one input row in each of the C pieces
+  int64_t p0 = 0, p1 = 0;                 // input rows the previous slab's buffer holds
+  for (int64_t s = 0; s < nslab; ++s) {
+    const int slot = (int)(s % kSlots);
+    const int64_t j0 = s * rows, j1 = (j0 + rows < L) ? j0 + rows : L;
+    const int64_t i0 = (j0 - ex.lo_rows < 0) ? 0 : j0 - ex.lo_rows;
+    const int64_t i1 = (j1 + ex.hi_rows > in.L) ? in.L : j1 + ex.hi_rows;
+    if (s >= kSlots) {
+      XG_CUDA(cudaStreamWaitEvent(w->s_h2d, w->e_done[slot], 0));  // kernels that read this slot's input
+      XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_down[slot], 0));    // downloads out of this slot's results
+    }
+    char* d_in = static_cast<char*>(w->in[slot].p);
+    const int64_t keep = (s > 0 && p1 > i0) ? p1 - i0 : 0;  // rows [i0, i0 + keep) are on the device already
+    if (keep)  // same in-order stream as the uploads
+      rc = copy_rows(d_in, (size_t)(i1 - i0) * row,
+                     static_cast<const char*>(w->in[(s - 1) % kSlots].p) + (size_t)(i0 - p0) * row,
+                     (size_t)(p1 - p0) * row, (size_t)keep * row, in.C, cudaMemcpyDeviceToDevice, w->s_h2d);
+    if (rc == XG_OK) rc = copy_slab(d_in + keep * row, i1 - i0, hin, in, i0 + keep, i1, es, true, w->s_h2d);
+    if (rc == XG_OK && ex.hin2) rc = copy_slab(w->in2[slot].p, j1 - j0, ex.hin2, ex.in2, j0, j1, es, true, w->s_h2d);
+    if (rc) return rc;
+    p0 = i0;
+    p1 = i1;
+    XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
+    XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[slot], 0));
+    void* d_out[kMaxOut];
+    for (int k = 0; k < nout; ++k) d_out[k] = w->out[slot][k].p;
+    const SlabBufs bufs{d_in,
+                        ex.hin2 ? w->in2[slot].p : nullptr,
+                        ex.scratch_row_bytes ? w->scratch.p : nullptr,
+                        {ex.plane_row_bytes ? w->plane[0].p : nullptr, ex.plane_row_bytes ? w->plane[1].p : nullptr},
+                        d_out};
+    rc = launch(j0, j1, i0, i1, bufs, w->s_k);
+    if (rc) return rc;
+    XG_CUDA(cudaEventRecord(w->e_done[slot], w->s_k));
+    XG_CUDA(cudaStreamWaitEvent(w->s_d2h, w->e_done[slot], 0));
+    for (int k = 0; rc == XG_OK && k < nout; ++k)
+      rc = copy_slab(d_out[k], j1 - j0, hout[k], out[k], j0, j1, es, false, w->s_d2h);
+    if (rc) return rc;
+    XG_CUDA(cudaEventRecord(w->e_down[slot], w->s_d2h));
+  }
+  for (cudaStream_t st : {w->s_d2h, w->s_k, w->s_h2d}) XG_CUDA(cudaStreamSynchronize(st));
   return XG_OK;
 }
 
 namespace {
 
+int workspace_bytes(const char* who, int device, int64_t* bytes) {
+  if (!bytes) return xg_fail(XG_EINVAL, std::string(who) + ": null pointer");
+  *bytes = 0;
+  Workspace* w = nullptr;
+  {
+    std::lock_guard<std::mutex> reg(g_registry);
+    w = find_workspace(device);
+  }
+  if (!w) return XG_OK;
+  std::lock_guard<std::mutex> lock(w->mu);
+  w->each_buf([&](Workspace::Buf& b) { *bytes += (int64_t)b.cap; });
+  return XG_OK;
+}
+
+// ------------------------------------------------------------------------------ the stencil and pair entry points
 // The x term and the second field of xg_stencil_pair_host.  Its Call describes the term along `axis`
 // (op_b, lo_b, hi_b, bc_b, fill_b, pre_b) and `post`, and its `in` is field a, the slab input.
 struct PairTerm {
@@ -145,7 +298,7 @@ struct PairTerm {
   int subtract;
 };
 
-// The stencil call the slab loop runs, slab by slab.
+// The stencil arguments of a host stencil entry point.
 struct Call {
   int op, dtype;
   const void* in;
@@ -159,26 +312,9 @@ struct Call {
   const void* post;
   const int64_t* post_strides;
   int device;
-  const PairTerm* pair = nullptr;  // xg_stencil_pair_halo instead of xg_stencil2
 };
 
-enum { kHaloNone = 0, kHaloFold = 1, kHaloCopies = 2 };
 enum { kSrcField = 0, kSrcPartner = 1, kSrcFill = 2 };
-
-// What builds a slab's halo planes on s_k before its xg_stencil2 launch (none for xg_stencil2_host).
-struct HaloStage {
-  int kind = kHaloNone;
-  // kHaloFold: the folded north row of the slab is halo_hi, and halo_lo when the south edge is periodic
-  int seam_axis = 0, skip = 0, negate = 0;
-  int64_t mirror = 0, period = 1;
-  // kHaloCopies: strided copies into the lo / hi planes, described once for the whole field (dim-0 extent n0)
-  const void* partner = nullptr;
-  int64_t partner_row = 0;  // partner elements per dim-0 index
-  int ncopies = 0, cndim = 0;
-  const int *side = nullptr, *source = nullptr, *negate_c = nullptr;
-  const int64_t *dst_offset = nullptr, *src_offset = nullptr, *shapes = nullptr;
-  const int64_t *dst_strides = nullptr, *src_strides = nullptr;
-};
 
 // Argument checks shared by the host stencil entry points; no CUDA call.
 int validate_call(const char* who, const Call& c) {
@@ -234,9 +370,8 @@ int validate_fold(const char* who, const Call& c, int seam_axis, int skip, int64
 }
 
 // The checks xg_stencil_pair makes, plus those of the slab loop (dim 0 a batch dim), before any CUDA call.
-int validate_pair_call(const char* who, const Call& c) {
+int validate_pair_call(const char* who, const Call& c, const PairTerm& t) {
   const std::string w(who);
-  const PairTerm& t = *c.pair;
   if (!t.b) return xg_fail(XG_EINVAL, w + ": null pointer");
   int rc = validate_halo_call(who, c);
   if (rc) return rc;
@@ -254,248 +389,90 @@ int validate_pair_call(const char* who, const Call& c) {
   return XG_OK;
 }
 
-// Per-slab face-connection copies: rebase the whole-field copy list onto the slab buffers, `rows` high.
-int halo_copies(const HaloStage& h, int dtype, size_t es, void* const planes[2], const void* field,
-                const void* partner, const void* fill, int64_t rows, std::vector<void*>& dptr,
-                std::vector<const void*>& sptr, std::vector<int64_t>& shp, cudaStream_t st) {
-  for (int k = 0; k < h.ncopies; ++k) {
-    dptr[k] = (char*)planes[h.side[k]] + (size_t)h.dst_offset[k] * es;
-    const void* base = h.source[k] == kSrcField ? field : h.source[k] == kSrcPartner ? partner : fill;
-    sptr[k] = (const char*)base + (size_t)h.src_offset[k] * es;
-    shp[(size_t)k * h.cndim] = rows;
-  }
-  int rc = xg_strided_copy_batch(dtype, h.ncopies, dptr.data(), sptr.data(), h.cndim, shp.data(),
-                                 h.dst_strides, h.src_strides, h.negate_c, st);
-  if (rc != XG_ENOTIMPL) return rc;
-  for (int k = 0; k < h.ncopies; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
-    rc = xg_strided_copy(dtype, dptr[k], h.dst_strides + (size_t)k * h.cndim, sptr[k],
-                         h.src_strides + (size_t)k * h.cndim, h.cndim, shp.data() + (size_t)k * h.cndim,
-                         h.negate_c[k], st);
-    if (rc) return rc;
-  }
-  return XG_OK;
+// A slab's halo stage, on the kernel stream before its stencil launch: builds the slab's halo planes into b.plane
+// and points *hl / *hh at them.  `slab_shape` is the slab's shape, `pre` its rows of the pre-metric.
+typedef std::function<int(const SlabBufs& b, const int64_t* slab_shape, const void* pre, cudaStream_t st,
+                          const void** hl, const void** hh)>
+    HaloFn;
+
+// The fold's halo stage: the folded north row of the slab (of the field across the fold: the input, or the second
+// input of a pair) is halo_hi, and halo_lo too when the south edge is periodic (it wraps the row above the top).
+HaloFn fold_stage(const Call& c, bool of_in2, int seam_axis, int skip, int64_t mirror, int64_t period, int negate) {
+  return [=](const SlabBufs& b, const int64_t* slab_shape, const void* pre, cudaStream_t st, const void** hl,
+             const void** hh) {
+    *hh = b.plane[1];
+    if (c.lo && c.bc == XG_BC_PERIODIC) *hl = *hh;
+    return xg_fold_rows(c.dtype, of_in2 ? b.in2 : b.in, b.plane[1], c.ndim, slab_shape, c.axis, seam_axis, 1, 0, 1,
+                        skip, mirror, period, negate ? 1 : 0, pre, c.pre_strides, st);
+  };
 }
 
-// The slab loop of every host stencil entry point (arguments already validated).
-int run_slabs(const Call& c, const HaloStage& h) {
-  const int ndim = c.ndim, axis = c.axis, lo = c.lo, hi = c.hi, bc = c.bc;
-  const int64_t* shape = c.shape;
+// A stencil entry point on the open session: field c.in in slabs along dim 0, `partner` (field b of pair `t`, or the
+// partner vector component, `partner_row` elements per dim-0 index) beside it, the metrics uploaded whole.  Per slab
+// `halo` (when dim 0 is a batch dim) builds the halo planes, then one xg_stencil2 or xg_stencil_pair_halo launch.
+int stencil_host(Session& ss, const Call& c, const PairTerm* t, const void* partner, int64_t partner_row,
+                 const HaloFn& halo) {
   const size_t es = c.dtype == XG_F32 ? 4 : 8;
-  XG_CUDA(cudaSetDevice(c.device));
-  Workspace* w = nullptr;
-  int rc;
-  {
-    std::lock_guard<std::mutex> reg(g_ws_mutex);  // registry only
-    rc = get_workspace(c.device, &w);
-  }
-  if (rc) return rc;
-  std::lock_guard<std::mutex> lock(w->mu);
-
+  const int ndim = c.ndim, lo = c.lo;
+  const bool ax0 = c.axis == 0;
+  const int64_t n0 = c.shape[0];
   int64_t out_shape[XG_MAX_NDIM];
-  for (int d = 0; d < ndim; ++d) out_shape[d] = shape[d];
-  out_shape[axis] = shape[axis] + lo + hi - 1;
-  int64_t row_in = 1, row_out = 1;  // elements per index of dim 0
-  for (int d = 1; d < ndim; ++d) {
-    row_in *= shape[d];
-    row_out *= out_shape[d];
-  }
-  const int64_t n0_out = out_shape[0];
-  if (n0_out <= 0 || row_out == 0 || row_in == 0) return XG_OK;
-  const void* partner = c.pair ? c.pair->b : h.partner;
-  const int64_t partner_row = c.pair ? row_in : h.partner_row;
-  const bool ax0 = axis == 0;
+  for (int d = 0; d < ndim; ++d) out_shape[d] = c.shape[d];
+  out_shape[c.axis] = c.shape[c.axis] + c.lo + c.hi - 1;
+  const View3 vin = view3(ndim, c.shape, 0), vout = view3(ndim, out_shape, 0);
+  if (vout.L <= 0 || vout.R == 0 || vin.R == 0) return XG_OK;
 
-  // slab height along dim 0: ~128 MiB of input per slab, at least 4 slabs if possible
-  int64_t target_bytes = 128ll << 20;
-  if (const char* env = getenv("XG_HOST_SLAB_MB")) {  // tuning knob (benchmarks only)
-    const long mb = atol(env);
-    if (mb >= 1 && mb <= 4096) target_bytes = (int64_t)mb << 20;
-  }
-  int64_t rows = target_bytes / (int64_t)(row_in * es);
-  if (rows < 1) rows = 1;
-  if (rows > (n0_out + 3) / 4) rows = (n0_out + 3) / 4;
-  if (rows < 1) rows = 1;
-  if (ax0 && bc == XG_BC_EXTRAPOLATE && (lo || hi)) {
-    // the extrapolated halo is 2 A[edge] - A[next]: the slab that touches an edge of the axis must hold two
-    // source planes, i.e. no one-row slab at either end (a one-row tail is merged by growing the slab height)
-    if (rows < 2) rows = 2;
-    while (rows < n0_out && n0_out % rows == 1) ++rows;
-    if (rows > n0_out) rows = n0_out;
-  }
-  const int64_t nslab = xg_ceil_div(n0_out, rows);
-  const int64_t in_rows_max = ax0 ? rows + 1 : rows;
+  const void *d_pre, *d_post, *d_pre_a = nullptr;
+  const void* wrap[2] = {nullptr, nullptr};  // periodic halo planes along dim 0: plane n0 - 1 below, plane 0 above
+  const size_t plane = (size_t)vin.R * es;
+  int rc = ss.upload(kAuxPre, c.pre, c.pre ? operand_span(c.pre_strides, c.shape, ndim, es) : 0, &d_pre);
+  if (rc == XG_OK)
+    rc = ss.upload(kAuxPost, c.post, c.post ? operand_span(c.post_strides, out_shape, ndim, es) : 0, &d_post);
+  if (rc == XG_OK && t && t->pre_a)
+    rc = ss.upload(kAuxPreA, t->pre_a, operand_span(t->pre_a_strides, c.shape, ndim, es), &d_pre_a);
+  if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && lo)
+    rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
+  if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && c.hi) rc = ss.upload(kAuxWrapHi, c.in, plane, &wrap[1]);
+  if (rc == XG_OK) rc = ss.fence();
+  if (rc) return rc;
 
-  for (int i = 0; i < kSlots; ++i) {
-    size_t have_in = w->slab_in_bytes, have_out = w->slab_out_bytes, have_p = w->partner_bytes;
-    rc = ensure(&w->d_in[i], &have_in, (size_t)(in_rows_max * row_in) * es);
-    if (rc) return rc;
-    rc = ensure(&w->d_out[i], &have_out, (size_t)(rows * row_out) * es);
-    if (rc) return rc;
-    if (partner) {
-      rc = ensure(&w->d_partner[i], &have_p, (size_t)(rows * partner_row) * es);
-      if (rc) return rc;
-    }
-    if (i == kSlots - 1) {
-      w->slab_in_bytes = have_in;
-      w->slab_out_bytes = have_out;
-      w->partner_bytes = have_p;
-    }
+  PipeExtra ex;
+  if (ax0) {  // result rows [j0, j1) read planes [j0 - lo, j1 - lo] of the padded field
+    ex.lo_rows = lo;
+    ex.hi_rows = 1 - lo;
+    ex.edge_pairs = c.bc == XG_BC_EXTRAPOLATE && (lo || c.hi);
   }
-  // (all three slots share one recorded capacity: grow them together)
-  // metrics: uploaded whole, once
-  const void* hm[3] = {c.pre, c.post, c.pair ? c.pair->pre_a : nullptr};
-  const int64_t* ms[3] = {c.pre_strides, c.post_strides, c.pair ? c.pair->pre_a_strides : nullptr};
-  const int64_t* mshape[3] = {shape, out_shape, shape};
-  for (int k = 0; k < 3; ++k) {
-    if (!hm[k]) continue;
-    const size_t span = operand_span(ms[k], mshape[k], ndim, es);
-    rc = ensure(&w->d_metric[k], &w->metric_bytes[k], span);
-    if (rc) return rc;
-    XG_CUDA(cudaMemcpyAsync(w->d_metric[k], hm[k], span, cudaMemcpyHostToDevice, w->s_h2d));
+  if (partner) {
+    ex.hin2 = partner;
+    ex.in2 = View3{1, n0, partner_row};
   }
-  // exterior halo planes when dim 0 is the operated axis and the halo is data (periodic wrap)
-  const char* hin = static_cast<const char*>(c.in);
-  char* hout = static_cast<char*>(c.out);
-  const int64_t n0 = shape[0];
-  const bool wrap_planes = ax0 && bc == XG_BC_PERIODIC && c.pre == nullptr;
-  if (wrap_planes) {
-    size_t hb = w->halo_bytes;
-    for (int k = 0; k < 2; ++k) {
-      size_t have = hb;
-      rc = ensure(&w->d_halo[k], &have, (size_t)row_in * es);
-      if (rc) return rc;
-      if (k == 1) w->halo_bytes = have;
+  if (halo) ex.plane_row_bytes = (size_t)(vin.R / c.shape[c.axis]) * es;
+  int64_t sshape[XG_MAX_NDIM];
+  for (int d = 0; d < ndim; ++d) sshape[d] = c.shape[d];
+  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
+    sshape[0] = i1 - i0;
+    const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(i0 * c.pre_strides[0]) * es : nullptr;
+    const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * c.post_strides[0]) * es : nullptr;
+    // along dim 0 a slab pads only the edges of the field its planes reach
+    const int slo = ax0 ? j0 - lo < 0 : lo, shi = ax0 ? j1 - lo + 1 > n0 : c.hi;
+    const void* hl = slo ? wrap[0] : nullptr;
+    const void* hh = shi ? wrap[1] : nullptr;
+    if (halo) {
+      const int rc2 = halo(b, sshape, pm, st, &hl, &hh);
+      if (rc2) return rc2;
     }
-    if (lo)  // below the first plane sits the last plane
-      XG_CUDA(cudaMemcpyAsync(w->d_halo[0], hin + (size_t)(n0 - 1) * row_in * es, row_in * es,
-                              cudaMemcpyHostToDevice, w->s_h2d));
-    if (hi)
-      XG_CUDA(cudaMemcpyAsync(w->d_halo[1], hin, row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
-  }
-  // per-slab halo planes (dim 0 is not the operated axis): one pair, built and read in order on s_k
-  std::vector<void*> dptr(h.ncopies);
-  std::vector<const void*> sptr(h.ncopies);
-  std::vector<int64_t> shp(h.shapes ? h.shapes : (const int64_t*)nullptr,
-                           h.shapes ? h.shapes + (size_t)h.ncopies * h.cndim : (const int64_t*)nullptr);
-  if (h.kind != kHaloNone) {
-    const int64_t plane_row = row_in / shape[axis];
-    size_t hb = w->halo_bytes;
-    for (int k = 0; k < 2; ++k) {
-      size_t have = hb;
-      rc = ensure(&w->d_halo[k], &have, (size_t)(rows * plane_row) * es);
-      if (rc) return rc;
-      if (k == 1) w->halo_bytes = have;
+    if (t) {
+      const char* am = d_pre_a ? static_cast<const char*>(d_pre_a) + (size_t)(i0 * t->pre_a_strides[0]) * es : nullptr;
+      return xg_stencil_pair_halo(c.dtype, b.in, b.in2, b.out[0], ndim, sshape, t->op_a, t->lo_a, t->hi_a, t->bc_a,
+                                  t->fill_a, am, t->pre_a_strides, c.axis, c.op, lo, c.hi, c.bc, c.fill_value, pm,
+                                  c.pre_strides, t->subtract, qm, c.post_strides, hl, hh, st);
     }
-    bool fill = false;
-    for (int k = 0; k < h.ncopies; ++k) fill = fill || h.source[k] == kSrcFill;
-    if (fill) {
-      rc = ensure(&w->d_const, &w->const_bytes, es);
-      if (rc) return rc;
-      const float f32 = (float)c.fill_value;  // pageable: staged before cudaMemcpyAsync returns
-      XG_CUDA(cudaMemcpyAsync(w->d_const, es == 4 ? (const void*)&f32 : (const void*)&c.fill_value, es,
-                              cudaMemcpyHostToDevice, w->s_h2d));
-    }
-  }
-  XG_CUDA(cudaEventRecord(w->e_up[0], w->s_h2d));
-  XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[0], 0));  // metrics + halo planes before any kernel
-
-  int64_t slab_shape[XG_MAX_NDIM];
-  for (int d = 0; d < ndim; ++d) slab_shape[d] = shape[d];
-
-  int64_t prev_last_row = -1;          // global index of the last plane of the previous slab
-  const char* prev_last_ptr = nullptr;  // ... and where it sits on the device
-  for (int64_t s = 0; s < nslab; ++s) {
-    const int slot = (int)(s % kSlots);
-    const int64_t j0 = s * rows;                                  // first output row of the slab
-    const int64_t j1 = (j0 + rows < n0_out) ? j0 + rows : n0_out;  // one past the last
-    // input rows needed: non-operated dim 0 -> [j0, j1); operated -> P[j0 .. j1] i.e.
-    // source rows [j0 - lo, j1 - lo] clipped to [0, n0)
-    int64_t i0 = j0, i1 = j1;
-    int slab_lo = lo, slab_hi = hi;
-    if (ax0) {
-      i0 = j0 - lo;
-      i1 = j1 - lo + 1;
-      slab_lo = 0;
-      slab_hi = 0;
-      if (i0 < 0) { i0 = 0; slab_lo = 1; }
-      if (i1 > n0) { i1 = n0; slab_hi = 1; }
-    }
-    // slot reuse: the previous D2H out of this slot must have drained, and the kernel that read
-    // the slot's input must have finished before we overwrite it
-    if (s >= kSlots) {
-      XG_CUDA(cudaStreamWaitEvent(w->s_h2d, w->e_done[slot], 0));
-      XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_down[slot], 0));
-    }
-    if (ax0 && s > 0 && prev_last_row == i0 && i1 - i0 > 1) {
-      // consecutive slabs of the operated axis overlap by exactly one plane: carry it over on the
-      // device (same in-order stream as the uploads) instead of sending it over PCIe again
-      XG_CUDA(cudaMemcpyAsync(w->d_in[slot], prev_last_ptr, (size_t)row_in * es,
-                              cudaMemcpyDeviceToDevice, w->s_h2d));
-      XG_CUDA(cudaMemcpyAsync((char*)w->d_in[slot] + (size_t)row_in * es,
-                              hin + (size_t)(i0 + 1) * row_in * es,
-                              (size_t)(i1 - i0 - 1) * row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
-    } else {
-      XG_CUDA(cudaMemcpyAsync(w->d_in[slot], hin + (size_t)i0 * row_in * es,
-                              (size_t)(i1 - i0) * row_in * es, cudaMemcpyHostToDevice, w->s_h2d));
-    }
-    if (partner)
-      XG_CUDA(cudaMemcpyAsync(w->d_partner[slot], static_cast<const char*>(partner) + (size_t)(i0 * partner_row) * es,
-                              (size_t)((i1 - i0) * partner_row) * es, cudaMemcpyHostToDevice, w->s_h2d));
-    prev_last_row = i1 - 1;
-    prev_last_ptr = (const char*)w->d_in[slot] + (size_t)(i1 - 1 - i0) * row_in * es;
-    XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
-    XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[slot], 0));
-
-    slab_shape[0] = i1 - i0;
-    const char* pm = (const char*)w->d_metric[0];
-    const char* qm = (const char*)w->d_metric[1];
-    if (c.pre) pm += (size_t)(i0 * c.pre_strides[0]) * es;
-    if (c.post) qm += (size_t)(j0 * c.post_strides[0]) * es;
-    const char* am = (const char*)w->d_metric[2];
-    if (c.pair && c.pair->pre_a) am += (size_t)(i0 * c.pair->pre_a_strides[0]) * es;
-    const void* hl = nullptr;
-    const void* hh = nullptr;
-    if (ax0 && wrap_planes) {
-      if (slab_lo) hl = w->d_halo[0];
-      if (slab_hi) hh = w->d_halo[1];
-    }
-    if (h.kind == kHaloFold) {
-      rc = xg_fold_rows(c.dtype, c.pair ? w->d_partner[slot] : w->d_in[slot], w->d_halo[1], ndim, slab_shape, axis,
-                        h.seam_axis, 1, 0, 1, h.skip, h.mirror, h.period, h.negate, c.pre ? pm : nullptr,
-                        c.pre_strides, w->s_k);
-      hh = w->d_halo[1];
-      if (lo && bc == XG_BC_PERIODIC) hl = hh;  // a periodic south edge wraps the row above the top
-    } else if (h.kind == kHaloCopies) {
-      rc = halo_copies(h, c.dtype, es, w->d_halo, w->d_in[slot], w->d_partner[slot], w->d_const, i1 - i0,
-                       dptr, sptr, shp, w->s_k);
-      if (lo) hl = w->d_halo[0];
-      if (hi) hh = w->d_halo[1];
-    }
-    if (rc == XG_OK && c.pair) {
-      const PairTerm& t = *c.pair;
-      rc = xg_stencil_pair_halo(c.dtype, w->d_in[slot], w->d_partner[slot], w->d_out[slot], ndim, slab_shape, t.op_a,
-                                t.lo_a, t.hi_a, t.bc_a, t.fill_a, t.pre_a ? am : nullptr, t.pre_a_strides, axis, c.op,
-                                lo, hi, bc, c.fill_value, c.pre ? pm : nullptr, c.pre_strides, t.subtract,
-                                c.post ? qm : nullptr, c.post_strides, hl, hh, w->s_k);
-    } else if (rc == XG_OK) {
-      rc = xg_stencil2(c.op, c.dtype, w->d_in[slot], w->d_out[slot], ndim, slab_shape, axis, slab_lo, slab_hi,
-                       (slab_lo || slab_hi) ? bc : XG_BC_NONE, c.fill_value, c.pre ? pm : nullptr,
-                       c.pre_strides, c.post ? qm : nullptr, c.post_strides, hl, hh, w->s_k);
-    }
-    if (rc) {
-      cudaDeviceSynchronize();
-      return rc;
-    }
-    XG_CUDA(cudaEventRecord(w->e_done[slot], w->s_k));
-    XG_CUDA(cudaStreamWaitEvent(w->s_d2h, w->e_done[slot], 0));
-    XG_CUDA(cudaMemcpyAsync(hout + (size_t)j0 * row_out * es, w->d_out[slot],
-                            (size_t)(j1 - j0) * row_out * es, cudaMemcpyDeviceToHost, w->s_d2h));
-    XG_CUDA(cudaEventRecord(w->e_down[slot], w->s_d2h));
-  }
-  XG_CUDA(cudaStreamSynchronize(w->s_d2h));
-  XG_CUDA(cudaStreamSynchronize(w->s_k));
-  XG_CUDA(cudaStreamSynchronize(w->s_h2d));
-  return XG_OK;
+    return xg_stencil2(c.op, c.dtype, b.in, b.out[0], ndim, sshape, c.axis, slo, shi,
+                       (slo || shi) ? c.bc : XG_BC_NONE, c.fill_value, pm, c.pre_strides, qm, c.post_strides, hl, hh,
+                       st);
+  };
+  void* outs[1] = {c.out};
+  return ss.run(es, c.in, vin, 1, outs, &vout, launch, ex);
 }
 
 // lowest and highest element a strided copy of `shape` touches from `offset`
@@ -510,6 +487,30 @@ void copy_extent(int64_t offset, const int64_t* strides, const int64_t* shape, i
 }
 
 }  // namespace
+}  // namespace xg_host
+
+using namespace xg_host;
+
+extern "C" int xg_host_workspace_release(void) {
+  std::lock_guard<std::mutex> reg(g_registry);
+  for (Workspace* w : g_ws) {
+    std::lock_guard<std::mutex> lock(w->mu);  // not while a call streams through it
+    cudaSetDevice(w->device);
+    w->each_buf([](Workspace::Buf& b) {
+      if (b.p) cudaFree(b.p);
+      b = Workspace::Buf();
+    });
+  }
+  return XG_OK;
+}
+
+extern "C" int xg_host_workspace_bytes(int device, int64_t* bytes) {
+  return workspace_bytes("xg_host_workspace_bytes", device, bytes);
+}
+
+extern "C" int xg_host_pipe_workspace_bytes(int device, int64_t* bytes) {
+  return workspace_bytes("xg_host_pipe_workspace_bytes", device, bytes);
+}
 
 extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, int ndim,
                                 const int64_t* shape, int axis, int lo, int hi, int bc,
@@ -520,7 +521,9 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
                pre_metric, pre_strides, post_metric, post_strides, device};
   int rc = validate_call("xg_stencil2_host", c);
   if (rc) return rc;
-  return run_slabs(c, HaloStage{});
+  Session ss;
+  rc = ss.open(device);
+  return rc ? rc : stencil_host(ss, c, nullptr, nullptr, 0, nullptr);
 }
 
 extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
@@ -534,14 +537,9 @@ extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* ou
   int rc = validate_halo_call(who, c);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
   if (rc) return rc;
-  HaloStage h;
-  h.kind = kHaloFold;
-  h.seam_axis = seam_axis;
-  h.skip = skip;
-  h.mirror = mirror;
-  h.period = period;
-  h.negate = negate ? 1 : 0;
-  return run_slabs(c, h);
+  Session ss;
+  rc = ss.open(device);
+  return rc ? rc : stencil_host(ss, c, nullptr, nullptr, 0, fold_stage(c, false, seam_axis, skip, mirror, period, negate));
 }
 
 extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, const void* partner,
@@ -579,6 +577,7 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
     }
   }
   int64_t covered[2] = {0, 0};
+  bool fill = false;
   for (int k = 0; k < ncopies; ++k) {
     const int64_t* sh = shapes + (size_t)k * copy_ndim;
     const int64_t* ds = dst_strides + (size_t)k * copy_ndim;
@@ -589,6 +588,7 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
     if (source[k] < kSrcField || source[k] > kSrcFill)
       return xg_fail(XG_EINVAL, at + "source must be 0 (field), 1 (partner) or 2 (fill constant)");
     if (source[k] == kSrcPartner && !partner) return xg_fail(XG_EINVAL, at + "reads a partner that was not given");
+    fill = fill || source[k] == kSrcFill;
     int64_t cells = 1;
     for (int d = 0; d < copy_ndim; ++d) {
       if (sh[d] < 0) return xg_fail(XG_EINVAL, at + "negative extent");
@@ -612,37 +612,42 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   // the copies write disjoint cells, so together they must cover each padded plane exactly once
   if ((lo && covered[0] != n0 * plane_row) || (hi && covered[1] != n0 * plane_row))
     return xg_fail(XG_EINVAL, who + ": the copies do not cover the halo planes");
-  HaloStage h;
-  h.kind = kHaloCopies;
-  h.partner = partner;
-  h.partner_row = partner_row;
-  h.ncopies = ncopies;
-  h.cndim = copy_ndim;
-  h.side = side;
-  h.source = source;
-  h.negate_c = negate;
-  h.dst_offset = dst_offset;
-  h.src_offset = src_offset;
-  h.shapes = shapes;
-  h.dst_strides = dst_strides;
-  h.src_strides = src_strides;
-  return run_slabs(c, h);
-}
 
-extern "C" int xg_host_workspace_bytes(int device, int64_t* bytes) {
-  if (!bytes) return xg_fail(XG_EINVAL, "xg_host_workspace_bytes: null pointer");
-  *bytes = 0;
-  Workspace* w = nullptr;
-  {
-    std::lock_guard<std::mutex> reg(g_ws_mutex);
-    for (Workspace* x : g_ws)
-      if (x->device == device) w = x;
-  }
-  if (!w) return XG_OK;
-  std::lock_guard<std::mutex> lock(w->mu);
-  *bytes = (int64_t)(kSlots * (w->slab_in_bytes + w->slab_out_bytes + w->partner_bytes) + w->metric_bytes[0] +
-                     w->metric_bytes[1] + w->metric_bytes[2] + 2 * w->halo_bytes + w->const_bytes);
-  return XG_OK;
+  Session ss;
+  rc = ss.open(device);
+  if (rc) return rc;
+  const size_t es = dtype == XG_F32 ? 4 : 8;
+  const void* d_fill = nullptr;
+  const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
+  if (fill) rc = ss.upload(kAuxFill, es == 4 ? (const void*)&f32 : (const void*)&fill_value, es, &d_fill);
+  if (rc) return rc;
+  // the whole-field copy list rebased onto each slab's buffers, `rows` high
+  std::vector<void*> dptr(ncopies);
+  std::vector<const void*> sptr(ncopies);
+  std::vector<int64_t> shp(shapes ? shapes : (const int64_t*)nullptr,
+                           shapes ? shapes + (size_t)ncopies * copy_ndim : (const int64_t*)nullptr);
+  auto copies = [&](const SlabBufs& b, const int64_t* slab_shape, const void*, cudaStream_t st, const void** hl,
+                    const void** hh) -> int {
+    for (int k = 0; k < ncopies; ++k) {
+      dptr[k] = static_cast<char*>(b.plane[side[k]]) + (size_t)dst_offset[k] * es;
+      const void* base = source[k] == kSrcField ? b.in : source[k] == kSrcPartner ? b.in2 : d_fill;
+      sptr[k] = static_cast<const char*>(base) + (size_t)src_offset[k] * es;
+      shp[(size_t)k * copy_ndim] = slab_shape[0];
+    }
+    if (lo) *hl = b.plane[0];
+    if (hi) *hh = b.plane[1];
+    int rc2 = xg_strided_copy_batch(dtype, ncopies, dptr.data(), sptr.data(), copy_ndim, shp.data(), dst_strides,
+                                    src_strides, negate, st);
+    if (rc2 != XG_ENOTIMPL) return rc2;
+    for (int k = 0; k < ncopies; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
+      rc2 = xg_strided_copy(dtype, dptr[k], dst_strides + (size_t)k * copy_ndim, sptr[k],
+                            src_strides + (size_t)k * copy_ndim, copy_ndim, shp.data() + (size_t)k * copy_ndim,
+                            negate[k], st);
+      if (rc2) return rc2;
+    }
+    return XG_OK;
+  };
+  return stencil_host(ss, c, nullptr, partner, partner_row, copies);
 }
 
 extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
@@ -652,10 +657,12 @@ extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, voi
                                     const void* post, const int64_t* post_strides, int device) {
   const PairTerm t{b, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, subtract};
   const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
-               pre_b, pre_b_strides, post, post_strides, device, &t};
-  int rc = validate_pair_call("xg_stencil_pair_host", c);
+               pre_b, pre_b_strides, post, post_strides, device};
+  int rc = validate_pair_call("xg_stencil_pair_host", c, t);
   if (rc) return rc;
-  return run_slabs(c, HaloStage{});
+  Session ss;
+  rc = ss.open(device);
+  return rc ? rc : stencil_host(ss, c, &t, b, view3(ndim, shape, 0).R, nullptr);
 }
 
 extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, void* out, int ndim,
@@ -668,16 +675,13 @@ extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b
   const char* who = "xg_stencil_pair_host_fold";
   const PairTerm t{b, op_a, lo_a, hi_a, bc_a, fill_a, pre_a, pre_a_strides, subtract};
   const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
-               pre_b, pre_b_strides, post, post_strides, device, &t};
-  int rc = validate_pair_call(who, c);
+               pre_b, pre_b_strides, post, post_strides, device};
+  int rc = validate_pair_call(who, c, t);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
   if (rc) return rc;
-  HaloStage h;
-  h.kind = kHaloFold;
-  h.seam_axis = seam_axis;
-  h.skip = skip;
-  h.mirror = mirror;
-  h.period = period;
-  h.negate = negate ? 1 : 0;
-  return run_slabs(c, h);
+  Session ss;
+  rc = ss.open(device);
+  return rc ? rc
+            : stencil_host(ss, c, &t, b, view3(ndim, shape, 0).R,
+                           fold_stage(c, true, seam_axis, skip, mirror, period, negate));
 }

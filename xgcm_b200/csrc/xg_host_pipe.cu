@@ -1,7 +1,6 @@
-// Host-buffer entry points beyond xg_stencil2_host: the SAME three-stream slab pipeline
-//     H2D(slab s+1)  ||  kernel(s)(slab s)  ||  D2H(slab s-1)
-// generalised to (a) several results per uploaded slab and (b) slabs cut along a dimension that is
-// not the outermost one (strided 2-D copies), so that every device entry point has a host twin:
+// Host-buffer entry points beyond the stencils of xg_host.cu, on the same slab engine (xg_host.cuh), with
+// (a) several results per uploaded slab and (b) slabs cut along a dimension that is not the outermost one
+// (strided 2-D copies), so that every device entry point has a host twin:
 //
 //   xg_stencil2_host_multi   one field up, K (op, axis, shift, boundary) results down: a `Grid.diff` +
 //                            `Grid.interp` sweep over X, Y, Z moves the field over PCIe once, not six
@@ -15,6 +14,8 @@
 // contiguous elements -> one cudaMemcpy2DAsync each way.  Lines along the operated axis stay whole, so
 // no halo exchange between slabs is needed and summation order is untouched.  xg_cumscan_host and
 // xg_wreduce_host cut the first non-operated dim, and upload their metric / weight whole, once.
+// xg_stencil2_host_multi cuts dim 0; results operated along it read the rows around each slab, which the
+// engine carries over from the previous slab on the device.
 //
 // The two transform twins pick the outermost non-operated dim of extent > 1 one index of which (its phi,
 // theta, theta-bounds scratch and result bytes together) fits the slab budget, else the innermost one, so
@@ -23,250 +24,14 @@
 // is the pipe's second streamed input: it goes up in the same slab window as phi into its own per-slot
 // buffers.  A broadcast theta (a 1-D coordinate, (T, Z+1, 1, 1), ...) is uploaded whole once.  Theta given
 // at cell centres (xg_vinterp_conservative_host's theta_at_centers) becomes its n + 1 bounds on the device:
-// one xg_stencil2(interp, lo = hi = 1, extend) along the axis per slab into a per-slot scratch buffer (once,
-// into an aux buffer, for a broadcast theta) -- the center -> outer shift of grid.interp(theta, axis,
+// one xg_stencil2(interp, lo = hi = 1, extend) along the axis per slab into the workspace's scratch buffer
+// (once, into an aux buffer, for a broadcast theta) -- the center -> outer shift of grid.interp(theta, axis,
 // padding="extend"), so the bounds are the ones that call would give.
-//
-// Workspaces (device slabs, streams, events) are cached per device and guarded by a per-device mutex:
-// calls on different GPUs run concurrently, calls on one GPU serialise (they would fight for PCIe anyway).
-#include <stdlib.h>
+#include "xg_host.cuh"
 
-#include <functional>
-#include <mutex>
-#include <vector>
-
-#include "xg_common.cuh"
+using namespace xg_host;
 
 namespace {
-
-constexpr int kSlots = 3;
-constexpr int kMaxOut = 8;
-constexpr int kMaxAux = 4;
-
-struct PipeWorkspace {
-  int device = -1;
-  std::mutex mu;
-  size_t in_cap[kSlots] = {0, 0, 0};
-  void* d_in[kSlots] = {nullptr, nullptr, nullptr};
-  size_t in2_cap[kSlots] = {0, 0, 0};
-  void* d_in2[kSlots] = {nullptr, nullptr, nullptr};  // second streamed input (a dense theta field)
-  size_t scr_cap[kSlots] = {0, 0, 0};
-  void* d_scr[kSlots] = {nullptr, nullptr, nullptr};  // per-slab scratch (theta bounds made from centres)
-  size_t out_cap[kSlots][kMaxOut] = {};
-  void* d_out[kSlots][kMaxOut] = {};
-  size_t aux_cap[kMaxAux] = {0, 0, 0, 0};
-  void* d_aux[kMaxAux] = {nullptr, nullptr, nullptr, nullptr};
-  cudaStream_t s_h2d = nullptr, s_k = nullptr, s_d2h = nullptr;
-  cudaEvent_t e_up[kSlots], e_done[kSlots], e_down[kSlots], e_aux;
-  bool ready = false;
-};
-
-std::mutex g_reg_mutex;
-std::vector<PipeWorkspace*> g_pipes;
-
-#define XG_CUDA(call)                                                               \
-  do {                                                                              \
-    cudaError_t e_ = (call);                                                        \
-    if (e_ != cudaSuccess)                                                          \
-      return xg_fail(XG_ECUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
-  } while (0)
-
-int ensure(void** p, size_t* have, size_t want) {
-  if (*have >= want && *p) return XG_OK;
-  if (*p) XG_CUDA(cudaFree(*p));
-  *p = nullptr;
-  *have = 0;
-  if (want == 0) return XG_OK;
-  XG_CUDA(cudaMalloc(p, want));
-  *have = want;
-  return XG_OK;
-}
-
-int get_pipe(int device, PipeWorkspace** out) {
-  std::lock_guard<std::mutex> lock(g_reg_mutex);
-  for (PipeWorkspace* w : g_pipes)
-    if (w->device == device) {
-      *out = w;
-      return XG_OK;
-    }
-  PipeWorkspace* w = new PipeWorkspace();
-  w->device = device;
-  g_pipes.push_back(w);
-  *out = w;
-  return XG_OK;
-}
-
-int init_pipe(PipeWorkspace* w) {  // caller holds w->mu and has set the device
-  if (w->ready) return XG_OK;
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_h2d, cudaStreamNonBlocking));
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_k, cudaStreamNonBlocking));
-  XG_CUDA(cudaStreamCreateWithFlags(&w->s_d2h, cudaStreamNonBlocking));
-  for (int i = 0; i < kSlots; ++i) {
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_up[i], cudaEventDisableTiming));
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_done[i], cudaEventDisableTiming));
-    XG_CUDA(cudaEventCreateWithFlags(&w->e_down[i], cudaEventDisableTiming));
-  }
-  XG_CUDA(cudaEventCreateWithFlags(&w->e_aux, cudaEventDisableTiming));
-  w->ready = true;
-  return XG_OK;
-}
-
-size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size_t es) {
-  int64_t last = 0;
-  for (int d = 0; d < ndim; ++d)
-    if (shape[d] > 1) last += (shape[d] - 1) * strides[d];
-  return (size_t)(last + 1) * es;
-}
-
-// [C][L][R] view of a C-contiguous array around the slab dimension (extent L)
-struct View3 {
-  int64_t C, L, R;
-};
-
-View3 view3(int ndim, const int64_t* shape, int sd) {
-  View3 v{1, ndim ? shape[sd] : 1, 1};
-  for (int d = 0; d < sd; ++d) v.C *= shape[d];
-  for (int d = sd + 1; d < ndim; ++d) v.R *= shape[d];
-  return v;
-}
-
-// rows [j0, j1) of the slab dim <-> a dense [C][j1-j0][R] device block
-int copy_slab(void* dev, const void* host_base, const View3& v, int64_t j0, int64_t j1, size_t es, bool to_device,
-              cudaStream_t st) {
-  const size_t width = (size_t)(j1 - j0) * v.R * es;
-  if (width == 0 || v.C == 0) return XG_OK;
-  const char* h = static_cast<const char*>(host_base) + (size_t)j0 * v.R * es;
-  const size_t hpitch = (size_t)v.L * v.R * es;
-  if (v.C == 1) {
-    if (to_device) XG_CUDA(cudaMemcpyAsync(dev, h, width, cudaMemcpyHostToDevice, st));
-    else XG_CUDA(cudaMemcpyAsync(const_cast<char*>(h), dev, width, cudaMemcpyDeviceToHost, st));
-    return XG_OK;
-  }
-  if (to_device) XG_CUDA(cudaMemcpy2DAsync(dev, width, h, hpitch, width, (size_t)v.C, cudaMemcpyHostToDevice, st));
-  else XG_CUDA(cudaMemcpy2DAsync(const_cast<char*>(h), hpitch, dev, width, width, (size_t)v.C, cudaMemcpyDeviceToHost, st));
-  return XG_OK;
-}
-
-int64_t slab_budget_bytes() {
-  int64_t target_bytes = 128ll << 20;
-  if (const char* env = getenv("XG_HOST_SLAB_MB")) {  // tuning knob (benchmarks only)
-    const long mb = atol(env);
-    if (mb >= 1 && mb <= 4096) target_bytes = (int64_t)mb << 20;
-  }
-  return target_bytes;
-}
-
-// rows of a slab dim of extent L whose one row (index) moves `row_bytes`
-int64_t slab_rows(int64_t L, int64_t row_bytes, int64_t extra_rows) {
-  int64_t rows = row_bytes > 0 ? slab_budget_bytes() / row_bytes : L;
-  if (rows < 1) rows = 1;
-  if (rows > (L + 3) / 4) rows = (L + 3) / 4;  // at least 4 slabs when the dim allows: overlap
-  if (rows < 1 + extra_rows) rows = 1 + extra_rows;
-  return rows;
-}
-
-// Optional parts of a pipeline: a second host input that goes up in the same slab window as the first, rows
-// [j0, j1) without halo, into per-slot buffers (its own [C][L][R] view, same L); a per-slot device scratch of
-// `scratch_row_bytes` per slab row; the bytes one slab row moves, which size the slabs (0: the first input's).
-struct PipeExtra {
-  const void* hin2 = nullptr;
-  View3 in2{0, 0, 0};
-  size_t scratch_row_bytes = 0;
-  int64_t row_bytes = 0;
-};
-
-struct SlabBufs {  // device buffers of the slot a slab runs in
-  void* in;
-  void* in2;      // the second input's rows, nullptr without one
-  void* scratch;  // nullptr without scratch
-  void* const* out;
-};
-
-// launch(j0, j1, i0, i1, bufs, stream): kernels for output rows [j0, j1) given input rows [i0, i1)
-typedef std::function<int(int64_t, int64_t, int64_t, int64_t, const SlabBufs&, cudaStream_t)> LaunchFn;
-
-// The pipeline.  `halo` = extra input rows wanted on each side of a slab (0, or 1 when some result is
-// operated along the slab dim).  Result k has view out[k] with the same L as the input.
-int run_pipe(PipeWorkspace* w, size_t es, const void* hin, const View3& in, int nout, void* const* hout,
-             const View3* out, int halo, const LaunchFn& launch, const PipeExtra& ex = PipeExtra()) {
-  if (in.L == 0 || in.C == 0 || in.R == 0) return XG_OK;
-  const int64_t rows = slab_rows(in.L, ex.row_bytes > 0 ? ex.row_bytes : in.C * in.R * (int64_t)es, 0);
-  const int64_t nslab = xg_ceil_div(in.L, rows);
-  for (int i = 0; i < kSlots; ++i) {
-    int rc = ensure(&w->d_in[i], &w->in_cap[i], (size_t)(in.C * (rows + 2 * halo) * in.R) * es);
-    if (rc) return rc;
-    if (ex.hin2) rc = ensure(&w->d_in2[i], &w->in2_cap[i], (size_t)(ex.in2.C * rows * ex.in2.R) * es);
-    if (rc) return rc;
-    if (ex.scratch_row_bytes) rc = ensure(&w->d_scr[i], &w->scr_cap[i], ex.scratch_row_bytes * (size_t)rows);
-    if (rc) return rc;
-    for (int k = 0; k < nout; ++k) {
-      rc = ensure(&w->d_out[i][k], &w->out_cap[i][k], (size_t)(out[k].C * rows * out[k].R) * es);
-      if (rc) return rc;
-    }
-  }
-  for (int64_t s = 0; s < nslab; ++s) {
-    const int slot = (int)(s % kSlots);
-    const int64_t j0 = s * rows, j1 = (j0 + rows < in.L) ? j0 + rows : in.L;
-    const int64_t i0 = (j0 - halo < 0) ? 0 : j0 - halo, i1 = (j1 + halo > in.L) ? in.L : j1 + halo;
-    if (s >= kSlots) {
-      XG_CUDA(cudaStreamWaitEvent(w->s_h2d, w->e_done[slot], 0));  // kernels that read this slot's input
-      XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_down[slot], 0));    // downloads out of this slot's results
-    }
-    int rc = copy_slab(w->d_in[slot], hin, in, i0, i1, es, true, w->s_h2d);
-    if (rc) return rc;
-    if (ex.hin2) rc = copy_slab(w->d_in2[slot], ex.hin2, ex.in2, j0, j1, es, true, w->s_h2d);
-    if (rc) return rc;
-    XG_CUDA(cudaEventRecord(w->e_up[slot], w->s_h2d));
-    XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_up[slot], 0));
-    const SlabBufs bufs{w->d_in[slot], ex.hin2 ? w->d_in2[slot] : nullptr,
-                        ex.scratch_row_bytes ? w->d_scr[slot] : nullptr, w->d_out[slot]};
-    rc = launch(j0, j1, i0, i1, bufs, w->s_k);
-    if (rc) {
-      cudaDeviceSynchronize();
-      return rc;
-    }
-    XG_CUDA(cudaEventRecord(w->e_done[slot], w->s_k));
-    XG_CUDA(cudaStreamWaitEvent(w->s_d2h, w->e_done[slot], 0));
-    for (int k = 0; k < nout; ++k) {
-      rc = copy_slab(w->d_out[slot][k], hout[k], out[k], j0, j1, es, false, w->s_d2h);
-      if (rc) return rc;
-    }
-    XG_CUDA(cudaEventRecord(w->e_down[slot], w->s_d2h));
-  }
-  XG_CUDA(cudaStreamSynchronize(w->s_d2h));
-  XG_CUDA(cudaStreamSynchronize(w->s_k));
-  XG_CUDA(cudaStreamSynchronize(w->s_h2d));
-  return XG_OK;
-}
-
-// upload a small broadcast operand whole (aux slot `slot`); *dev = its device address (nullptr if absent)
-int upload_aux(PipeWorkspace* w, int slot, const void* host, size_t bytes, const void** dev) {
-  *dev = nullptr;
-  if (!host) return XG_OK;
-  int rc = ensure(&w->d_aux[slot], &w->aux_cap[slot], bytes);
-  if (rc) return rc;
-  XG_CUDA(cudaMemcpyAsync(w->d_aux[slot], host, bytes, cudaMemcpyHostToDevice, w->s_h2d));
-  *dev = w->d_aux[slot];
-  return XG_OK;
-}
-
-int aux_fence(PipeWorkspace* w) {  // kernels must see the aux uploads
-  XG_CUDA(cudaEventRecord(w->e_aux, w->s_h2d));
-  XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_aux, 0));
-  return XG_OK;
-}
-
-struct Session {  // device selected, workspace locked and initialised
-  PipeWorkspace* w = nullptr;
-  std::unique_lock<std::mutex> lock;
-  int open(int device) {
-    int rc = get_pipe(device, &w);
-    if (rc) return rc;
-    lock = std::unique_lock<std::mutex>(w->mu);
-    XG_CUDA(cudaSetDevice(device));
-    return init_pipe(w);
-  }
-};
 
 int first_free_dim(int ndim, int axis) { return (ndim == 1) ? -1 : (axis == 0 ? 1 : 0); }
 
@@ -372,9 +137,9 @@ int check_theta(const char* fn, int ndim, const int64_t* tshape, const int64_t* 
 }
 
 // Build the plan once the session is open; theta holds `tn` values along the axis (n + 1 bounds, n centres, or the
-// n levels of the linear twin).  A broadcast theta goes up whole into aux slot 0; plan_theta_bounds makes the bounds
+// n levels of the linear twin).  A broadcast theta goes up whole (kAuxTheta); plan_theta_bounds makes the bounds
 // of one that holds centres.
-int plan_theta(PipeWorkspace* w, ThetaPlan* p, int dtype, const void* theta, const int64_t* strides, int centers,
+int plan_theta(Session& ss, ThetaPlan* p, int dtype, const void* theta, const int64_t* strides, int centers,
                int64_t tn, int ndim, const int64_t* shape, int axis) {
   p->dtype = dtype;
   p->es = dtype == XG_F32 ? 4 : 8;
@@ -386,28 +151,29 @@ int plan_theta(PipeWorkspace* w, ThetaPlan* p, int dtype, const void* theta, con
   p->bshape[axis] = p->centers ? tn + 1 : tn;
   p->dense = theta_is_dense(ndim, p->tshape, strides);
   if (p->dense) return XG_OK;
-  int rc = upload_aux(w, 0, theta, operand_span(strides, p->tshape, ndim, p->es), &p->d_bcast);
+  int rc = ss.upload(kAuxTheta, theta, operand_span(strides, p->tshape, ndim, p->es), &p->d_bcast);
   if (rc) return rc;
   for (int d = 0; d < ndim; ++d) p->bstrides[d] = strides[d];
   return XG_OK;
 }
 
-// the bounds of a broadcast theta held at centres, once, into aux slot 1, on the kernel stream (after aux_fence)
-int plan_theta_bounds(PipeWorkspace* w, ThetaPlan* p, const int64_t* strides) {
+// the bounds of a broadcast theta held at centres, once, into kAuxThetaBounds, on the kernel stream (after the fence)
+int plan_theta_bounds(Session& ss, ThetaPlan* p, const int64_t* strides) {
   if (p->dense || !p->centers) return XG_OK;
   int64_t cshape[XG_MAX_NDIM], cb[XG_MAX_NDIM];
   compact_shape(p->ndim, p->tshape, strides, cshape);
   for (int d = 0; d < p->ndim; ++d) cb[d] = cshape[d];
   cb[p->axis] = p->bshape[p->axis];
-  int rc = ensure(&w->d_aux[1], &w->aux_cap[1], (size_t)numel(p->ndim, cb) * p->es);
+  void* bounds = nullptr;
+  int rc = ss.aux(kAuxThetaBounds, (size_t)numel(p->ndim, cb) * p->es, &bounds);
   if (rc) return rc;
-  rc = xg_stencil2(XG_OP_INTERP, p->dtype, p->d_bcast, w->d_aux[1], p->ndim, cshape, p->axis, 1, 1, XG_BC_EXTEND,
-                   0.0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, w->s_k);
+  rc = xg_stencil2(XG_OP_INTERP, p->dtype, p->d_bcast, bounds, p->ndim, cshape, p->axis, 1, 1, XG_BC_EXTEND,
+                   0.0, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, ss.kernel_stream());
   if (rc) return rc;
   dense_strides(p->ndim, cb, p->bstrides);
   for (int d = 0; d < p->ndim; ++d)
     if (cb[d] == 1) p->bstrides[d] = 0;  // broadcast again over phi's extent
-  p->d_bcast = w->d_aux[1];
+  p->d_bcast = bounds;
   return XG_OK;
 }
 
@@ -449,35 +215,6 @@ TransformViews transform_views(int ndim, const int64_t* shape, int axis, int64_t
 
 }  // namespace
 
-void xg_host_pipe_release() {
-  std::lock_guard<std::mutex> lock(g_reg_mutex);
-  for (PipeWorkspace* w : g_pipes) {
-    std::lock_guard<std::mutex> l2(w->mu);
-    cudaSetDevice(w->device);
-    for (int i = 0; i < kSlots; ++i) {
-      if (w->d_in[i]) cudaFree(w->d_in[i]);
-      w->d_in[i] = nullptr;
-      w->in_cap[i] = 0;
-      if (w->d_in2[i]) cudaFree(w->d_in2[i]);
-      w->d_in2[i] = nullptr;
-      w->in2_cap[i] = 0;
-      if (w->d_scr[i]) cudaFree(w->d_scr[i]);
-      w->d_scr[i] = nullptr;
-      w->scr_cap[i] = 0;
-      for (int k = 0; k < kMaxOut; ++k) {
-        if (w->d_out[i][k]) cudaFree(w->d_out[i][k]);
-        w->d_out[i][k] = nullptr;
-        w->out_cap[i][k] = 0;
-      }
-    }
-    for (int i = 0; i < kMaxAux; ++i) {
-      if (w->d_aux[i]) cudaFree(w->d_aux[i]);
-      w->d_aux[i] = nullptr;
-      w->aux_cap[i] = 0;
-    }
-  }
-}
-
 // ---------------------------------------------------------------------------------------------------
 extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const void* in, void* const* out, int ndim,
                                       const int64_t* shape, const int* axis, const int* lo, const int* hi,
@@ -490,7 +227,7 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
     return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: dtype must be XG_F32 or XG_F64");
   if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: bad ndim");
   const size_t es = dtype == XG_F32 ? 4 : 8;
-  bool any0 = false;
+  PipeExtra ex;  // each slab reads the rows around it that its results along dim 0 need
   for (int k = 0; k < nout; ++k) {
     if (!out[k]) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: null result pointer");
     if (axis[k] < 0 || axis[k] >= ndim) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: axis out of range");
@@ -510,13 +247,13 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
                        "xg_stencil2_host for that result");
       if (bc[k] == XG_BC_EXTRAPOLATE)
         return xg_fail(XG_ENOTIMPL, "xg_stencil2_host_multi: extrapolate along the outermost dimension");
-      any0 = true;
+      if (lo[k] > ex.lo_rows) ex.lo_rows = lo[k];
+      if (hi[k] > ex.hi_rows) ex.hi_rows = hi[k];
     }
   }
   Session ss;
   int rc = ss.open(device);
   if (rc) return rc;
-  PipeWorkspace* w = ss.w;
 
   const View3 vin = view3(ndim, shape, 0);
   View3 vout[kMaxOut];
@@ -534,11 +271,9 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
   for (int k = 0; k < nout; ++k) need_wrap = need_wrap || (axis[k] == 0 && bc[k] == XG_BC_PERIODIC);
   if (need_wrap) {
     const size_t pb = (size_t)vin.R * es;
-    rc = upload_aux(w, 0, static_cast<const char*>(in) + (size_t)(n0 - 1) * pb, pb, &d_wrap[0]);
-    if (rc) return rc;
-    rc = upload_aux(w, 1, in, pb, &d_wrap[1]);
-    if (rc) return rc;
-    rc = aux_fence(w);
+    rc = ss.upload(kAuxWrapLo, static_cast<const char*>(in) + (size_t)(n0 - 1) * pb, pb, &d_wrap[0]);
+    if (rc == XG_OK) rc = ss.upload(kAuxWrapHi, in, pb, &d_wrap[1]);
+    if (rc == XG_OK) rc = ss.fence();
     if (rc) return rc;
   }
   auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
@@ -573,7 +308,7 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
     }
     return XG_OK;
   };
-  return run_pipe(w, es, in, vin, nout, out, vout, any0 ? 1 : 0, launch);
+  return ss.run(es, in, vin, nout, out, vout, launch, ex);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -596,15 +331,14 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
   Session ss;
   int rc = ss.open(device);
   if (rc) return rc;
-  PipeWorkspace* w = ss.w;
   const int sd = first_free_dim(ndim, axis);
   const void* d_pre = nullptr;
   const void* d_post = nullptr;
-  if (pre_metric) rc = upload_aux(w, 0, pre_metric, operand_span(pre_strides, shape, ndim, es), &d_pre);
+  if (pre_metric) rc = ss.upload(kAuxPre, pre_metric, operand_span(pre_strides, shape, ndim, es), &d_pre);
   if (rc) return rc;
-  if (post_metric) rc = upload_aux(w, 1, post_metric, operand_span(post_strides, out_shape, ndim, es), &d_post);
+  if (post_metric) rc = ss.upload(kAuxPost, post_metric, operand_span(post_strides, out_shape, ndim, es), &d_post);
   if (rc) return rc;
-  rc = aux_fence(w);
+  rc = ss.fence();
   if (rc) return rc;
   if (sd < 0) {  // 1-D: one slab = the whole line
     const View3 v{1, 1, shape[0]}, vo{1, 1, out_shape[0]};
@@ -613,7 +347,7 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
       return xg_cumscan(dtype, b.in, b.out[0], ndim, shape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, d_pre,
                         pre_strides, d_post, post_strides, skipna, st);
     };
-    return run_pipe(w, es, in, v, 1, outs, &vo, 0, launch);
+    return ss.run(es, in, v, 1, outs, &vo, launch);
   }
   const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
   void* outs[1] = {out};
@@ -628,7 +362,7 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
     return xg_cumscan(dtype, b.in, b.out[0], ndim, sshape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, pm,
                       pre_strides, qm, post_strides, skipna, st);
   };
-  return run_pipe(w, es, in, vin, 1, outs, &vout, 0, launch);
+  return ss.run(es, in, vin, 1, outs, &vout, launch);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -643,11 +377,10 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
   Session ss;
   int rc = ss.open(device);
   if (rc) return rc;
-  PipeWorkspace* w = ss.w;
   const void* d_w = nullptr;
-  if (weight) rc = upload_aux(w, 0, weight, operand_span(w_strides, shape, ndim, es), &d_w);
+  if (weight) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
   if (rc) return rc;
-  rc = aux_fence(w);
+  rc = ss.fence();
   if (rc) return rc;
   const int sd = first_free_dim(ndim, axis);
   void* outs[1] = {out};
@@ -656,7 +389,7 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
     auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
       return xg_wreduce(dtype, b.in, d_w, w_strides, b.out[0], ndim, shape, axis, mode, skipna, st);
     };
-    return run_pipe(w, es, in, v, 1, outs, &vo, 0, launch);
+    return ss.run(es, in, v, 1, outs, &vo, launch);
   }
   // result shape = shape without `axis`; the slab dim keeps its extent
   int64_t out_shape[XG_MAX_NDIM];
@@ -675,7 +408,7 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
     if (wm) wm += (size_t)(j0 * w_strides[sd]) * es;
     return xg_wreduce(dtype, b.in, wm, w_strides, b.out[0], ndim, sshape, axis, mode, skipna, st);
   };
-  return run_pipe(w, es, in, vin, 1, outs, &vout, 0, launch);
+  return ss.run(es, in, vin, 1, outs, &vout, launch);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -694,19 +427,18 @@ extern "C" int xg_vinterp_linear_host(int dtype, const void* phi, const void* th
   Session ss;
   int rc = ss.open(device);
   if (rc) return rc;
-  PipeWorkspace* w = ss.w;
-  // theta: a dense field streams beside phi, a broadcast one is uploaded whole (aux 0); target whole (aux 1)
+  // theta: a dense field streams beside phi, a broadcast one is uploaded whole; target whole
   ThetaPlan tp;
-  rc = plan_theta(w, &tp, dtype, theta, theta_strides, 0, shape[axis], ndim, shape, axis);
+  rc = plan_theta(ss, &tp, dtype, theta, theta_strides, 0, shape[axis], ndim, shape, axis);
   if (rc) return rc;
   const void* d_target = nullptr;
   int64_t tshape[XG_MAX_NDIM];
   for (int d = 0; d < ndim; ++d) tshape[d] = shape[d];
   tshape[axis] = m;
   const size_t tbytes = target_strides ? operand_span(target_strides, tshape, ndim, es) : (size_t)m * es;
-  rc = upload_aux(w, 1, target, tbytes ? tbytes : es, &d_target);
+  rc = ss.upload(kAuxTarget, target, tbytes ? tbytes : es, &d_target);
   if (rc) return rc;
-  rc = aux_fence(w);
+  rc = ss.fence();
   if (rc) return rc;
   const TransformViews tv = transform_views(ndim, shape, axis, m, tp, theta);
   tp.sd = tv.sd;
@@ -725,7 +457,7 @@ extern "C" int xg_vinterp_linear_host(int dtype, const void* phi, const void* th
     return xg_vinterp_linear(dtype, b.in, th, th_strides, tg, target_strides, m, b.out[0], ndim, sshape, axis,
                              mask_edges, bypass_checks, logarithmic, st);
   };
-  return run_pipe(w, es, phi, tv.vin, 1, outs, &tv.vout, 0, launch, tv.ex);
+  return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -765,17 +497,16 @@ extern "C" int xg_vinterp_conservative_host(int dtype, const void* phi, const vo
   Session ss;
   rc = ss.open(device);
   if (rc) return rc;
-  PipeWorkspace* w = ss.w;
-  // theta: streamed (dense) or whole in aux 0 (its bounds in aux 1 at centres); bins whole in aux 2
+  // theta: streamed (dense) or whole (its bounds made on the device at centres); bins whole
   ThetaPlan tp;
-  rc = plan_theta(w, &tp, dtype, theta, theta_strides, theta_at_centers, tshape[axis], ndim, shape, axis);
+  rc = plan_theta(ss, &tp, dtype, theta, theta_strides, theta_at_centers, tshape[axis], ndim, shape, axis);
   if (rc) return rc;
   const void* d_bins = nullptr;
-  rc = upload_aux(w, 2, target_bins, (size_t)m * es, &d_bins);
+  rc = ss.upload(kAuxTarget, target_bins, (size_t)m * es, &d_bins);
   if (rc) return rc;
-  rc = aux_fence(w);
+  rc = ss.fence();
   if (rc) return rc;
-  rc = plan_theta_bounds(w, &tp, theta_strides);
+  rc = plan_theta_bounds(ss, &tp, theta_strides);
   if (rc) return rc;
   const TransformViews tv = transform_views(ndim, shape, axis, m - 1, tp, theta);
   tp.sd = tv.sd;
@@ -790,26 +521,5 @@ extern "C" int xg_vinterp_conservative_host(int dtype, const void* phi, const vo
     return xg_vinterp_conservative(dtype, b.in, th, th_strides, d_bins, m, flip_out, b.out[0], ndim, sshape, axis,
                                    st);
   };
-  return run_pipe(w, es, phi, tv.vin, 1, outs, &tv.vout, 0, launch, tv.ex);
-}
-
-extern "C" int xg_host_pipe_workspace_bytes(int device, int64_t* bytes) {
-  if (!bytes) return xg_fail(XG_EINVAL, "xg_host_pipe_workspace_bytes: null pointer");
-  *bytes = 0;
-  PipeWorkspace* w = nullptr;
-  {
-    std::lock_guard<std::mutex> reg(g_reg_mutex);
-    for (PipeWorkspace* x : g_pipes)
-      if (x->device == device) w = x;
-  }
-  if (!w) return XG_OK;
-  std::lock_guard<std::mutex> lock(w->mu);
-  size_t total = 0;
-  for (int i = 0; i < kSlots; ++i) {
-    total += w->in_cap[i] + w->in2_cap[i] + w->scr_cap[i];
-    for (int k = 0; k < kMaxOut; ++k) total += w->out_cap[i][k];
-  }
-  for (int i = 0; i < kMaxAux; ++i) total += w->aux_cap[i];
-  *bytes = (int64_t)total;
-  return XG_OK;
+  return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex);
 }
