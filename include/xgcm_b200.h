@@ -434,6 +434,33 @@ XG_API int xg_vinterp_conservative_host(int dtype, const void* phi, const void* 
                                  const void* target_bins, int64_t m, int flip_out, void* out, int ndim,
                                  const int64_t* shape, int axis, int device);
 
+/*
+ * Host-buffer twin of xg_stencil_multi (same semantics and argument checks, HOST pointers, `device` instead of a
+ * stream; synchronous): one xg_stencil_multi launch per slab.  Slabs are cut along the outermost dim of extent > 1
+ * that is not operated, so every operated line is whole in a slab.  When every dim of extent > 1 is operated, the
+ * outermost of them is cut: each slab reads the row next to it, an inner slab edge has no boundary condition and
+ * the field's own ends keep the call's; an outer / inner shift or a periodic boundary along that dim gives
+ * XG_ENOTIMPL (use xg_stencil_multi).  Every argument is checked before any CUDA call.
+ */
+XG_API int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
+                                 const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
+                                 const double* fill_value, int device);
+
+/*
+ * Weighted sum (XG_REDUCE_SUM) or mean (XG_REDUCE_MEAN) of a HOST field over the `naxes` >= 2 distinct dims
+ * `axes`, bit for bit the device sequence of Grid.integrate / average: one xg_wreduce per dim, innermost first,
+ * `weight` (optional, broadcast via w_strides) in the first only; a mean reduces the sum and the valid weights
+ * (XG_REDUCE_WVALID, then plain sums with skipna = 0) side by side and divides once (XG_BIN_DIVNZ).  out: shape
+ * without `axes` (one value when every dim is reduced).  Slabs are cut along the outermost dim of extent > 1 that is
+ * not reduced; with none, along the outermost dim of extent > 1, whose per-slab partials stay on the device for
+ * the launches along it, run once.  A weight that spans the slab dim (a dense array of its own extents) streams
+ * beside the field; otherwise it is uploaded whole.  XG_ENOTIMPL for an empty reduced dim, or when no reduced dim
+ * of extent > 1 lies inside the slab dim (use xg_wreduce_host).  Every argument is checked before any CUDA call.
+ */
+XG_API int xg_wreduce_host_multi(int dtype, const void* in, const void* weight, const int64_t* w_strides,
+                                 void* out, int ndim, const int64_t* shape, int naxes, const int* axes, int mode,
+                                 int skipna, int device);
+
 /* Device bytes the one workspace of the *_host entry points holds on `device`: the same number as
  * xg_host_workspace_bytes, kept for callers of the multi, scan, reduce and transform twins. */
 XG_API int xg_host_pipe_workspace_bytes(int device, int64_t* bytes);

@@ -121,6 +121,14 @@ SIGNATURES = {
         C.c_int,
         [C.c_int, _vp, _vp, _i64p, C.c_int, _vp, C.c_int64, C.c_int, _vp, C.c_int, _i64p, C.c_int, C.c_int],
     ),
+    "xg_stencil_multi_host": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, _i32p, _i32p, _i32p, _i32p, _i32p, _f64p, C.c_int],
+    ),
+    "xg_wreduce_host_multi": (
+        C.c_int,
+        [C.c_int, _vp, _vp, _i64p, _vp, C.c_int, _i64p, C.c_int, _i32p, C.c_int, C.c_int, C.c_int],
+    ),
     "xg_host_pipe_workspace_bytes": (C.c_int, [C.c_int, _i64p]),
     "xg_host_workspace_release": (C.c_int, []),
     "xg_stencil_pair": (

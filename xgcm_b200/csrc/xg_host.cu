@@ -208,6 +208,12 @@ int Session::fence() {
 
 cudaStream_t Session::kernel_stream() const { return w_->s_k; }
 
+int Session::download(void* host, const void* dev, size_t bytes) {
+  XG_CUDA(cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, w_->s_k));
+  XG_CUDA(cudaStreamSynchronize(w_->s_k));
+  return XG_OK;
+}
+
 int Session::run(size_t es, const void* hin, const View3& in, int nout, void* const* hout, const View3* out,
                  const LaunchFn& launch, const PipeExtra& ex) {
   Workspace* w = w_;

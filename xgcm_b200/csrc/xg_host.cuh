@@ -24,6 +24,7 @@ enum Aux {
   kAuxTheta,        // a broadcast theta
   kAuxThetaBounds,  // its bounds, made on the device from centres
   kAuxTarget,       // target levels of xg_vinterp_linear_host, or the bins of xg_vinterp_conservative_host
+  kAuxPartial,      // per-slab partials of xg_wreduce_host_multi over every dim, and what their last launches make
   kNumAux
 };
 
@@ -74,6 +75,8 @@ class Session {
   int aux(Aux a, size_t bytes, void** dev);
   int fence();  // kernels on kernel_stream() see the uploads
   cudaStream_t kernel_stream() const;
+  // Copy `bytes` at `dev` to `host` after the kernels on kernel_stream(), and wait for it
+  int download(void* host, const void* dev, size_t bytes);
   // Stream `hin` (view `in`) through `launch` into the `nout` results hout[k] (view out[k]); the results share
   // one L, which may differ from the input's.
   int run(size_t es, const void* hin, const View3& in, int nout, void* const* hout, const View3* out,

@@ -5,8 +5,11 @@
 //   xg_stencil2_host_multi   one field up, K (op, axis, shift, boundary) results down: a `Grid.diff` +
 //                            `Grid.interp` sweep over X, Y, Z moves the field over PCIe once, not six
 //                            times (xgcm/grid.py:796-832 would re-read it per call).
+//   xg_stencil_multi_host    xgcm/grid.py:798-832 (a multi-axis diff / interp / min / max): one
+//                            xg_stencil_multi launch per slab
 //   xg_cumscan_host          xgcm/grid.py:1306-1414 on numpy-backed fields
 //   xg_wreduce_host          xgcm/grid.py:1598-1605, :1680-1685
+//   xg_wreduce_host_multi    the same over several dims: the device launch sequence per slab
 //   xg_vinterp_linear_host        xgcm/transform.py:233-249
 //   xg_vinterp_conservative_host  xgcm/transform.py:157-198 (k_vconserv per slab)
 //
@@ -16,6 +19,11 @@
 // xg_wreduce_host cut the first non-operated dim, and upload their metric / weight whole, once.
 // xg_stencil2_host_multi cuts dim 0; results operated along it read the rows around each slab, which the
 // engine carries over from the previous slab on the device.
+//
+// The two multi-axis twins cut the outermost dim of extent > 1 that is not operated, so every operated line is
+// whole in a slab.  When every dim of extent > 1 is operated, xg_stencil_multi_host cuts the outermost one and
+// reads the row next to each slab (as xg_stencil2_host_multi does along dim 0), and xg_wreduce_host_multi keeps
+// one partial per index of it on the device and runs the launches along it once, at the end.
 //
 // The two transform twins pick the outermost non-operated dim of extent > 1 one index of which (its phi,
 // theta, theta-bounds scratch and result bytes together) fits the slab budget, else the innermost one, so
@@ -50,8 +58,9 @@ void dense_strides(int ndim, const int64_t* shape, int64_t* strides) {  // C ord
   }
 }
 
-// theta is a dense C-contiguous array of `tshape` (dims of extent 1 aside): it streams beside phi
-bool theta_is_dense(int ndim, const int64_t* tshape, const int64_t* strides) {
+// a dense C-contiguous array of `tshape` (dims of extent 1 aside), which can stream beside the field (theta beside
+// phi, a weight beside the field it reduces)
+bool is_dense(int ndim, const int64_t* tshape, const int64_t* strides) {
   int64_t ds[XG_MAX_NDIM];
   dense_strides(ndim, tshape, ds);
   for (int d = 0; d < ndim; ++d)
@@ -124,7 +133,7 @@ int check_theta(const char* fn, int ndim, const int64_t* tshape, const int64_t* 
     return xg_fail(XG_EINVAL, std::string(fn) + ": theta must hold " + std::to_string(tshape[axis]) +
                                   (centers ? " cell-centre values" : " cell bounds") +
                                   " along the axis; it is broadcast along it");
-  if (centers && !theta_is_dense(ndim, tshape, strides)) {
+  if (centers && !is_dense(ndim, tshape, strides)) {
     int64_t cshape[XG_MAX_NDIM], cs[XG_MAX_NDIM];
     compact_shape(ndim, tshape, strides, cshape);
     dense_strides(ndim, cshape, cs);
@@ -149,7 +158,7 @@ int plan_theta(Session& ss, ThetaPlan* p, int dtype, const void* theta, const in
   for (int d = 0; d < ndim; ++d) p->tshape[d] = p->bshape[d] = shape[d];
   p->tshape[axis] = tn;
   p->bshape[axis] = p->centers ? tn + 1 : tn;
-  p->dense = theta_is_dense(ndim, p->tshape, strides);
+  p->dense = is_dense(ndim, p->tshape, strides);
   if (p->dense) return XG_OK;
   int rc = ss.upload(kAuxTheta, theta, operand_span(strides, p->tshape, ndim, p->es), &p->d_bcast);
   if (rc) return rc;
@@ -312,6 +321,104 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
 }
 
 // ---------------------------------------------------------------------------------------------------
+extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
+                                     const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
+                                     const double* fill_value, int device) {
+  const std::string who = "xg_stencil_multi_host";
+  if (!in || !out || !shape || !axes || !ops || !lo || !hi || !bc || !fill_value)
+    return xg_fail(XG_EINVAL, who + ": null pointer");
+  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, who + ": bad ndim");
+  if (naxes < 2 || naxes > 3) return xg_fail(XG_EINVAL, who + ": 2 or 3 axes (use xg_stencil2 for one)");
+  for (int k = 0; k < naxes; ++k) {
+    if (ops[k] < XG_OP_DIFF || ops[k] > XG_OP_MAX) return xg_fail(XG_EINVAL, who + ": unknown op");
+    if (ops[k] != ops[0])
+      return xg_fail(XG_ENOTIMPL, who + ": the fused kernel applies ONE operator along all axes "
+                                        "(what Grid.diff / interp / min / max do); chain xg_stencil2 for mixed ones");
+  }
+  if (in == out) return xg_fail(XG_EINVAL, who + ": in-place operation is not supported");
+  if (dtype != XG_F32 && dtype != XG_F64) return xg_fail(XG_EINVAL, who + ": dtype must be XG_F32 or XG_F64");
+  for (int d = 0; d < ndim; ++d)
+    if (shape[d] < 0) return xg_fail(XG_EINVAL, who + ": negative extent");
+  int app[XG_MAX_NDIM];  // application index of each dim, -1 where it is not operated
+  int64_t out_shape[XG_MAX_NDIM];
+  for (int d = 0; d < ndim; ++d) {
+    app[d] = -1;
+    out_shape[d] = shape[d];
+  }
+  for (int k = 0; k < naxes; ++k) {
+    const int d = axes[k];
+    if (d < 0 || d >= ndim) return xg_fail(XG_EINVAL, who + ": axis out of range");
+    if (app[d] >= 0) return xg_fail(XG_EINVAL, who + ": an axis may appear only once");
+    if (lo[k] < 0 || lo[k] > 1 || hi[k] < 0 || hi[k] > 1)
+      return xg_fail(XG_EINVAL, who + ": halo widths must be 0 or 1");
+    if ((lo[k] || hi[k]) && (bc[k] < XG_BC_PERIODIC || bc[k] > XG_BC_EXTEND))
+      return xg_fail(XG_EINVAL, who + ": each padded axis needs a periodic / fill / extend boundary");
+    if (shape[d] == 0) return xg_fail(XG_EINVAL, who + ": empty operated axis");
+    app[d] = k;
+    out_shape[d] = shape[d] + lo[k] + hi[k] - 1;
+  }
+  // slab dim: the outermost non-operated dim of extent > 1, whose slabs hold every operated line whole; else the
+  // outermost dim of extent > 1, an operated one (the dims in front of it have extent 1)
+  int sd = -1;
+  for (int d = 0; d < ndim && sd < 0; ++d)
+    if (app[d] < 0 && shape[d] > 1) sd = d;
+  for (int d = 0; d < ndim && sd < 0; ++d)
+    if (shape[d] > 1) sd = d;
+  if (sd < 0) sd = 0;
+  const int ka = app[sd];  // the application cut into slabs, -1 when none is
+  PipeExtra ex;
+  if (ka >= 0) {
+    // each slab reads the row next to it along the cut dim; xg_stencil_multi takes no halo planes, so only the
+    // field's own ends can be padded, and a slab of result rows must read as many input rows (lo + hi == 1)
+    if (lo[ka] + hi[ka] != 1)
+      return xg_fail(XG_ENOTIMPL, who + ": outer / inner shift along the cut dim (every dim of extent > 1 is "
+                                        "operated); use xg_stencil_multi");
+    if (bc[ka] == XG_BC_PERIODIC)
+      return xg_fail(XG_ENOTIMPL, who + ": periodic boundary along the cut dim (every dim of extent > 1 is "
+                                        "operated); use xg_stencil_multi");
+    ex.lo_rows = lo[ka];
+    ex.hi_rows = hi[ka];
+  }
+  int64_t total_out = 1;
+  for (int d = 0; d < ndim; ++d) total_out *= out_shape[d];
+  if (total_out == 0) return XG_OK;
+  const size_t es = dtype == XG_F32 ? 4 : 8;
+  const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
+  ex.row_bytes = (vin.C * vin.R + vout.C * vout.R) * (int64_t)es;
+  Session ss;
+  int rc = ss.open(device);
+  if (rc) return rc;
+  const int64_t n = shape[sd];
+  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
+    int64_t sshape[XG_MAX_NDIM];
+    int slo[3], shi[3], sbc[3];
+    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+    for (int k = 0; k < naxes; ++k) {
+      slo[k] = lo[k];
+      shi[k] = hi[k];
+      sbc[k] = bc[k];
+    }
+    const char* src = static_cast<const char*>(b.in);
+    if (ka >= 0) {
+      // result rows [j0, j1) need padded planes [j0, j1], i.e. input rows [j0 - lo, j1 - lo] clipped to the field:
+      // an inner slab edge reads its neighbour row, the field's own ends keep the call's boundary condition
+      int64_t s0 = j0 - lo[ka], s1 = j1 - lo[ka] + 1;
+      slo[ka] = shi[ka] = 0;
+      if (s0 < 0) { s0 = 0; slo[ka] = 1; }
+      if (s1 > n) { s1 = n; shi[ka] = 1; }
+      if (s0 < i0 || s1 > i1 || vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
+      if (!slo[ka] && !shi[ka]) sbc[ka] = XG_BC_NONE;
+      src += (size_t)(s0 - i0) * vin.R * es;
+      sshape[sd] = s1 - s0;
+    } else {
+      sshape[sd] = j1 - j0;
+    }
+    return xg_stencil_multi(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc, fill_value, st);
+  };
+  return ss.run(es, in, vin, 1, &out, &vout, launch, ex);
+}
+
+// ---------------------------------------------------------------------------------------------------
 extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,
                                int reverse, int trim, int pad_lo, int pad_hi, int bc, double fill_value,
                                const void* pre_metric, const int64_t* pre_strides, const void* post_metric,
@@ -409,6 +516,215 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
     return xg_wreduce(dtype, b.in, wm, w_strides, b.out[0], ndim, sshape, axis, mode, skipna, st);
   };
   return ss.run(es, in, vin, 1, outs, &vout, launch);
+}
+
+// ---------------------------------------------------------------------------------------------------
+extern "C" int xg_wreduce_host_multi(int dtype, const void* in, const void* weight, const int64_t* w_strides,
+                                     void* out, int ndim, const int64_t* shape, int naxes, const int* axes, int mode,
+                                     int skipna, int device) {
+  const std::string who = "xg_wreduce_host_multi";
+  if (!in || !out || !shape || !axes) return xg_fail(XG_EINVAL, who + ": null pointer");
+  if (dtype != XG_F32 && dtype != XG_F64) return xg_fail(XG_EINVAL, who + ": dtype must be XG_F32 or XG_F64");
+  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, who + ": bad ndim");
+  if (naxes < 2 || naxes > ndim)
+    return xg_fail(XG_EINVAL, who + ": between 2 and ndim axes (use xg_wreduce_host for one)");
+  if (mode != XG_REDUCE_SUM && mode != XG_REDUCE_MEAN)
+    return xg_fail(XG_EINVAL, who + ": mode must be XG_REDUCE_SUM or XG_REDUCE_MEAN");
+  if (weight && !w_strides) return xg_fail(XG_EINVAL, who + ": weight strides missing");
+  bool red[XG_MAX_NDIM] = {false};
+  for (int k = 0; k < naxes; ++k) {
+    if (axes[k] < 0 || axes[k] >= ndim) return xg_fail(XG_EINVAL, who + ": axis out of range");
+    if (red[axes[k]]) return xg_fail(XG_EINVAL, who + ": an axis may appear only once");
+    red[axes[k]] = true;
+  }
+  for (int d = 0; d < ndim; ++d) {
+    if (shape[d] < 0) return xg_fail(XG_EINVAL, who + ": negative extent");
+    if (weight && w_strides[d] < 0) return xg_fail(XG_EINVAL, who + ": negative weight stride");
+  }
+  int64_t out_numel = 1;
+  for (int d = 0; d < ndim; ++d)
+    if (!red[d]) out_numel *= shape[d];
+  if (out_numel == 0) return XG_OK;
+  for (int d = 0; d < ndim; ++d)
+    if (red[d] && shape[d] == 0) return xg_fail(XG_ENOTIMPL, who + ": empty reduced dim; use xg_wreduce");
+  const bool mean = mode == XG_REDUCE_MEAN;
+  const int mult = mean ? 2 : 1;  // a mean carries the sum and the valid weights side by side
+  const size_t es = dtype == XG_F32 ? 4 : 8;
+
+  // The launches of Grid.integrate / average on the device: one xg_wreduce per dim, innermost first, the weight in
+  // the first one only; a mean reduces sum and valid weights (WVALID) side by side, then divides once (DIVNZ).
+  int ord[XG_MAX_NDIM];
+  int nord = 0;
+  for (int d = ndim - 1; d >= 0; --d)
+    if (red[d]) ord[nord++] = d;
+  // Slab dim: the outermost non-reduced dim of extent > 1; every launch runs per slab.  With none (`whole`), slabs
+  // of the outermost dim of extent > 1 run the launches along the dims inside it; their partials, one value per
+  // index of the slab dim, stay on the device, and the launches along the slab dim and the extent-1 dims in front
+  // of it run once at the end.
+  int sd = -1;
+  for (int d = 0; d < ndim && sd < 0; ++d)
+    if (!red[d] && shape[d] > 1) sd = d;
+  const bool whole = sd < 0;
+  for (int d = 0; d < ndim && sd < 0; ++d)
+    if (shape[d] > 1) sd = d;
+  if (sd < 0) sd = 0;
+  int nslab = nord;  // launches (per chain) that run per slab
+  if (whole) {
+    nslab = 0;
+    while (nslab < nord && ord[nslab] > sd) ++nslab;
+    if (nslab == 0)
+      return xg_fail(XG_ENOTIMPL, who + ": no reduced dim of extent > 1 inside the slab dim; use xg_wreduce_host");
+  }
+  const int64_t L = shape[sd];
+  // elements per slab row of each per-slab launch's result, and of the scratch that holds them
+  int64_t rowel[XG_MAX_NDIM], scratch_el = 0;
+  {
+    int64_t c[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) c[d] = shape[d];
+    c[sd] = 1;
+    int cn = ndim;
+    for (int k = 0; k < nslab; ++k) {
+      for (int d = ord[k]; d + 1 < cn; ++d) c[d] = c[d + 1];
+      rowel[k] = numel(--cn, c);
+      if (k < nslab - 1 || (!whole && mean)) scratch_el += mult * rowel[k];
+    }
+  }
+  // the weight: streamed beside the field when it spans the slab dim (a dense array of its own extents), else whole
+  int64_t wshape[XG_MAX_NDIM];  // its own extents: 1 where it is broadcast
+  if (weight) compact_shape(ndim, shape, w_strides, wshape);
+  const bool stream_w = weight && wshape[sd] > 1 && is_dense(ndim, wshape, w_strides);
+
+  const View3 vin = view3(ndim, shape, sd);
+  View3 vout{1, L, 1};
+  if (!whole) {
+    int64_t oshape[XG_MAX_NDIM];
+    int nd_o = 0, sd_o = 0;
+    for (int d = 0; d < ndim; ++d) {
+      if (red[d]) continue;
+      if (d == sd) sd_o = nd_o;
+      oshape[nd_o++] = shape[d];
+    }
+    vout = view3(nd_o, oshape, sd_o);
+  }
+  PipeExtra ex;
+  if (stream_w) {
+    ex.hin2 = weight;
+    ex.in2 = view3(ndim, wshape, sd);
+  }
+  ex.scratch_row_bytes = (size_t)scratch_el * es;
+  ex.row_bytes = (vin.C * vin.R + (stream_w ? ex.in2.C * ex.in2.R : 0) + scratch_el +
+                  (whole ? 0 : vout.C * vout.R)) * (int64_t)es;
+
+  Session ss;
+  int rc = ss.open(device);
+  if (rc) return rc;
+  const void* d_w = nullptr;
+  if (weight && !stream_w) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
+  if (rc) return rc;
+  rc = ss.fence();
+  if (rc) return rc;
+  // `whole`: [sum partials (L)][valid-weight partials (L)], the results of the last launches, the mean
+  char* partial = nullptr;
+  int64_t partial_el = mult * L + 1;
+  if (whole) {
+    int64_t c[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) c[d] = shape[d];
+    int cn = ndim;
+    for (int k = 0; k < nord; ++k) {
+      for (int d = ord[k]; d + 1 < cn; ++d) c[d] = c[d + 1];
+      if (k >= nslab) partial_el += mult * numel(cn - 1, c);
+      --cn;
+    }
+    void* p = nullptr;
+    rc = ss.aux(kAuxPartial, (size_t)partial_el * es, &p);
+    if (rc) return rc;
+    partial = static_cast<char*>(p);
+  }
+  // launches k0 .. k1 - 1 of the chain on `cur` (cnd dims), from num_in (den_in: the valid weights of a mean), the
+  // weight with launch 0; the results of each go to the next free `scratch` elements, or to num_last / den_last
+  // for the last one when they are given
+  auto chain = [&](int k0, int k1, int64_t* cur, int cnd, const void* num_in, const void* den_in, const void* wp,
+                   const int64_t* ws, char* scratch, void* num_last, void* den_last, const void** num_out,
+                   const void** den_out, cudaStream_t st) -> int {
+    for (int k = k0; k < k1; ++k) {
+      const int64_t count = numel(cnd, cur) / cur[ord[k]];
+      void* nd = num_last;
+      void* dd = den_last;
+      if (k < k1 - 1 || !num_last) {
+        nd = scratch;
+        dd = mean ? scratch + (size_t)count * es : nullptr;
+        scratch += (size_t)(mult * count) * es;
+      }
+      int rc2;
+      if (k == 0) {
+        rc2 = mean ? xg_wreduce(dtype, num_in, wp, ws, dd, cnd, cur, ord[k], XG_REDUCE_WVALID, skipna, st) : XG_OK;
+        if (rc2 == XG_OK) rc2 = xg_wreduce(dtype, num_in, wp, ws, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
+      } else {
+        rc2 = xg_wreduce(dtype, num_in, nullptr, nullptr, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
+        if (rc2 == XG_OK && mean)
+          rc2 = xg_wreduce(dtype, den_in, nullptr, nullptr, dd, cnd, cur, ord[k], XG_REDUCE_SUM, 0, st);
+      }
+      if (rc2) return rc2;
+      num_in = nd;
+      den_in = dd;
+      for (int d = ord[k]; d + 1 < cnd; ++d) cur[d] = cur[d + 1];
+      --cnd;
+    }
+    *num_out = num_in;
+    *den_out = den_in;
+    return XG_OK;
+  };
+  // the mean: sum / valid weights, NaN where no weight is valid
+  auto divide = [&](const void* num, const void* den, void* res, int64_t count, cudaStream_t st) -> int {
+    const int64_t one = 1;
+    return xg_binary(XG_BIN_DIVNZ, dtype, num, den, &one, res, 1, &count, st);
+  };
+  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+    const int64_t rows = j1 - j0;
+    int64_t cur[XG_MAX_NDIM], ws[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) cur[d] = shape[d];
+    cur[sd] = rows;
+    const void* wp = nullptr;
+    if (stream_w) {  // the slab's own dense layout
+      int64_t c[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) c[d] = wshape[d];
+      c[sd] = rows;
+      dense_strides(ndim, c, ws);
+      for (int d = 0; d < ndim; ++d)
+        if (c[d] == 1) ws[d] = 0;
+      wp = b.in2;
+    } else if (d_w) {
+      for (int d = 0; d < ndim; ++d) ws[d] = w_strides[d];
+      wp = static_cast<const char*>(d_w) + (size_t)(j0 * w_strides[sd]) * es;
+    }
+    void* num_last = whole ? partial + (size_t)j0 * es : (mean ? nullptr : b.out[0]);
+    void* den_last = whole && mean ? partial + (size_t)(L + j0) * es : nullptr;
+    const void *num, *den;
+    int rc2 = chain(0, nslab, cur, ndim, b.in, nullptr, wp, wp ? ws : nullptr, static_cast<char*>(b.scratch),
+                    num_last, den_last, &num, &den, st);
+    if (rc2 || whole || !mean) return rc2;
+    return divide(num, den, b.out[0], rows * rowel[nslab - 1], st);
+  };
+  if (!whole) return ss.run(es, in, vin, 1, &out, &vout, launch, ex);
+  rc = ss.run(es, in, vin, 0, nullptr, &vout, launch, ex);
+  if (rc) return rc;
+  // the launches along the slab dim and the dims in front of it, once, on the partials
+  int64_t cur[XG_MAX_NDIM];
+  int cnd = 0;
+  for (int d = 0; d < ndim; ++d)
+    if (!(red[d] && d > sd)) cur[cnd++] = shape[d];
+  const void *num, *den;
+  char* next = partial + (size_t)(mult * L) * es;
+  rc = chain(nslab, nord, cur, cnd, partial, mean ? partial + (size_t)L * es : nullptr, nullptr, nullptr, next,
+             nullptr, nullptr, &num, &den, ss.kernel_stream());
+  if (rc) return rc;
+  if (mean) {
+    void* res = partial + (size_t)(partial_el - 1) * es;  // the last element
+    rc = divide(num, den, res, 1, ss.kernel_stream());
+    if (rc) return rc;
+    num = res;
+  }
+  return ss.download(out, num, es);
 }
 
 // ---------------------------------------------------------------------------------------------------

@@ -605,10 +605,20 @@ class Grid:
             rename[in_dim] = out_dim
         if array.shape[-1] < 32:
             return None  # tiny rows: the one-block-per-row kernel has nothing to chew on
-        x, was_host = as_device_tensor(array.data, self._device_for(array))
-        out = ops.stencil_multi(x, specs)
+        out = None
+        dev = self._device_for(array)
+        if not array.is_device and dev.type == "cuda" and np.asarray(array.data).dtype in (np.float32, np.float64):
+            # numpy-backed field: slabs stream through the GPU (xg_stencil_multi_host), so input, result and the
+            # device footprint need not fit in HBM together
+            try:
+                out = ops.stencil_multi_host(np.asarray(array.data), specs, device=dev.index)
+            except NotImplementedError:
+                out = None  # a cut along an operated dim the slabs cannot pad: the whole field on the device
+        if out is None:
+            x, was_host = as_device_tensor(array.data, dev)
+            out = result_like(ops.stencil_multi(x, specs), was_host)
         out_dims = tuple(rename.get(d, d) for d in array.dims)
-        res = DataArray(result_like(out, was_host), dims=out_dims, name=array.name, attrs=array.attrs)
+        res = DataArray(out, dims=out_dims, name=array.name, attrs=array.attrs)
         return _reattach_coords([res], self, None, set(rename.values()), [array])[0]
 
     def apply_many(self, da, requests, padding=None, fill_value=None):
@@ -1063,7 +1073,23 @@ class Grid:
             res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ != dims[0]), name=da.name)
             coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
             return self._wrap_out(res.assign_coords(coords), as_xarray)
-        x, _ = as_device_tensor(da.data, self._device_for(da))
+        dev = self._device_for(da)
+        if (host_input and len(set(dims)) == len(dims) > 1 and dev.type == "cuda"
+                and np.asarray(da.data).dtype in (np.float32, np.float64)):
+            # numpy-backed field, several axes: the launches below run per slab (xg_wreduce_host_multi), with a
+            # weight that spans the slab dim streamed beside the field
+            arr = np.asarray(da.data)
+            w_np = self._metric_host(weight, da.dims, arr.dtype)
+            try:
+                y = ops.wreduce_host_multi(arr, [da.get_axis_num(d) for d in dims], w_np, mode, bool(skipna),
+                                           device=dev.index)
+            except NotImplementedError:
+                y = None  # an empty reduced dim, or a single line: the whole field on the device
+            if y is not None:
+                res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ not in dims), name=da.name)
+                coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
+                return self._wrap_out(res.assign_coords(coords), as_xarray)
+        x, _ = as_device_tensor(da.data, dev)
         cur = da._replace(data=x)
         wt = self._metric_tensor(weight, cur.dims, x)
         # several axes: the first pass (innermost listed dim) applies the weights, the others are plain sums

@@ -847,6 +847,50 @@ def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: Optional[int] =
     return list(outs)
 
 
+def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, Optional[str], float]],
+                       device: Optional[int] = None) -> np.ndarray:
+    """Host twin of :func:`stencil_multi` (``xg_stencil_multi_host``): slabs of the outermost non-operated dim of
+    extent > 1 stream through the GPU, one fused launch each.  Raises NotImplementedError for what the slabs do not
+    cover (mixed operators; an outer / inner shift or a periodic boundary along the cut dim when every dim of extent
+    > 1 is operated) — callers then use :func:`stencil_multi`."""
+    import ctypes as C
+
+    lib = _capi.load()
+    x = _host_field(x, "field")
+    if not 2 <= len(specs) <= 3:
+        raise ValueError("stencil_multi fuses 2 or 3 axes")
+    shape = list(x.shape)
+    out_shape = list(shape)
+    axes, opc, los, his, bcs, fills = [], [], [], [], [], []
+    for axis, op, lo, hi, padding, fill in specs:
+        axis = _norm_axis(axis, x.ndim)
+        if op not in _capi.OPS:
+            raise ValueError(f"unknown op {op!r}")
+        if padding not in ("periodic", "fill", "extend", None):
+            raise NotImplementedError(f"fused multi-axis stencils support periodic / fill / extend, not {padding!r}")
+        if (lo or hi) and padding is None:
+            raise ValueError("no boundary condition was specified but the operation needs to pad the axis")
+        axes.append(axis)
+        opc.append(_capi.OPS[op])
+        los.append(int(lo))
+        his.append(int(hi))
+        bcs.append(_capi.BCS[padding] if (lo or hi) else 0)
+        fills.append(float(fill))
+        out_shape[axis] = shape[axis] + lo + hi - 1
+    if len(set(axes)) != len(axes):
+        raise ValueError("each axis may appear only once")
+    out = pinned_empty(out_shape, x.dtype)
+    n = len(specs)
+    IntArr, DblArr = C.c_int * n, C.c_double * n
+    dev = torch.cuda.current_device() if device is None else int(device)
+    if out.size:
+        rc = lib.xg_stencil_multi_host(
+            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), n,
+            IntArr(*axes), IntArr(*opc), IntArr(*los), IntArr(*his), IntArr(*bcs), DblArr(*fills), dev)
+        _capi.check(rc)
+    return out
+
+
 def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "none", pad_lo: int = 0,
                  pad_hi: int = 0, padding: Optional[str] = None, fill_value: float = 0.0,
                  pre: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None, skipna: bool = True,
@@ -890,6 +934,31 @@ def wreduce_host(x: np.ndarray, axis: int, weight: Optional[np.ndarray] = None, 
     if out.size and x.size:
         rc = lib.xg_wreduce_host(_capi.dtype_code(x.dtype), x.ctypes.data, w_ptr, w_st, out.ctypes.data, x.ndim,
                                  _capi.i64_array(shape), axis, _capi.REDUCE[mode], int(bool(skipna)), dev)
+        _capi.check(rc)
+    return out if out_shape else out.reshape(())
+
+
+def wreduce_host_multi(x: np.ndarray, axes: Sequence[int], weight: Optional[np.ndarray] = None, mode: str = "sum",
+                       skipna: bool = True, device: Optional[int] = None) -> np.ndarray:
+    """Weighted sum / mean of a host field over several ``axes`` (``xg_wreduce_host_multi``), bit for bit the
+    chain of :func:`wreduce` calls ``Grid.integrate`` / ``Grid.average`` run on the device.  Raises
+    NotImplementedError for what the slabs do not cover (an empty reduced dim, or no reduced dim of extent > 1
+    inside the slab dim) — callers then use :func:`wreduce`."""
+    import ctypes as C
+
+    lib = _capi.load()
+    x = _host_field(x, "field")
+    axes = [_norm_axis(a, x.ndim) for a in axes]
+    shape = list(x.shape)
+    out_shape = [s for d, s in enumerate(shape) if d not in axes]
+    out = pinned_empty(out_shape if out_shape else [1], x.dtype)
+    kw, w_ptr, w_st = _host_operand(weight, shape, x.dtype, "weight")
+    dev = torch.cuda.current_device() if device is None else int(device)
+    if out.size:
+        n = len(axes)
+        rc = lib.xg_wreduce_host_multi(_capi.dtype_code(x.dtype), x.ctypes.data, w_ptr, w_st, out.ctypes.data,
+                                       x.ndim, _capi.i64_array(shape), n, (C.c_int * n)(*axes), _capi.REDUCE[mode],
+                                       int(bool(skipna)), dev)
         _capi.check(rc)
     return out if out_shape else out.reshape(())
 
