@@ -383,8 +383,32 @@ XG_API int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, vo
 
 /* Device bytes the one workspace of the *_host entry points holds on `device` (slot buffers, halo planes,
  * scratch, whole-call operands such as metrics); 0 before the first call or after xg_host_workspace_release.
- * Same number as xg_host_pipe_workspace_bytes. */
+ * Same number as xg_host_pipe_workspace_bytes.  `device` is a device index: a group handle gives XG_EINVAL. */
 XG_API int xg_host_workspace_bytes(int device, int64_t* bytes);
+
+/*
+ * Host device groups: one *_host call spread over several GPUs.  xg_host_group registers the `n` device indices
+ * `devices` and writes a handle to *group, XG_HOST_GROUP_BASE + k, which no device index reaches; the same member
+ * list gives the same handle back.  A member may appear more than once: its blocks then take turns on that
+ * device's workspace.  Up to XG_HOST_GROUP_MAX groups of 1 .. XG_HOST_GROUP_MAX_MEMBERS members; XG_EINVAL past
+ * either cap, for a null pointer or a negative index (before any CUDA call), and for an index at or past
+ * cudaGetDeviceCount.  Groups live for the process.
+ *
+ * Every *_host entry point that streams slabs (xg_stencil2_host and its _multi / _fold / _connected variants,
+ * xg_stencil_multi_host, xg_stencil_pair_host[_fold], xg_cumscan_host, xg_wreduce_host[_multi] and both
+ * xg_vinterp_*_host) takes a handle in its `device` argument.  The result rows along the call's slab dim are cut
+ * into contiguous near-equal blocks, one per member (fewer when there are fewer rows), and each member streams
+ * its block on its own host thread through its own workspace, with the whole-call operands uploaded once per
+ * member.  Results are bit for bit those of a single device: the slabs run the same launches on the same rows.
+ * The call returns when every member has finished, with the first failing member's status (in member order) and
+ * message; the calling thread's xg_last_launch() is the first member's.  xg_wreduce_host_multi with every dim
+ * of extent > 1 reduced keeps its partials along the slab dim on one device and runs on the first member alone.
+ * An unknown handle gives XG_EINVAL before any CUDA call.
+ */
+#define XG_HOST_GROUP_BASE 1048576
+#define XG_HOST_GROUP_MAX 64
+#define XG_HOST_GROUP_MAX_MEMBERS 64
+XG_API int xg_host_group(int n, const int* devices, int* group);
 
 /*
  * One HOST field up, `nout` results down: result k = xg_stencil2(op[k], axis[k], lo[k], hi[k], bc[k],

@@ -21,6 +21,7 @@ TRIMS = {"none": 0, "drop_last": 1, "drop_first": 2}
 REDUCE = {"sum": 0, "mean": 1, "wvalid": 2}
 BINOPS = {"mul": 0, "div": 1, "add": 2, "sub": 3, "divnz": 4}
 XG_MAX_NDIM = 8
+XG_HOST_GROUP_BASE = 1048576  # handles of xg_host_group: XG_HOST_GROUP_BASE + k
 
 _EXC = {-1: ValueError, -2: NotImplementedError, -3: RuntimeError, -4: RuntimeError}
 
@@ -99,6 +100,7 @@ SIGNATURES = {
          _vp, _i64p, C.c_int, C.c_int, _i32p, _i32p, _i64p, _i64p, _i64p, _i64p, _i64p, _i32p, C.c_int],
     ),
     "xg_host_workspace_bytes": (C.c_int, [C.c_int, _i64p]),
+    "xg_host_group": (C.c_int, [C.c_int, _i32p, _i32p]),
     "xg_stencil2_host_multi": (
         C.c_int,
         [C.c_int, _i32p, C.c_int, _vp, _vpp, C.c_int, _i64p, _i32p, _i32p, _i32p, _i32p, _f64p, C.c_int],

@@ -22,6 +22,8 @@
 void xg_set_error(const std::string& msg);
 int xg_fail(int code, const std::string& msg);
 int xg_check_launch(const char* what);
+// the calling thread's xg_last_launch() label (a string literal), e.g. as a worker thread left it
+void xg_set_last_launch(const char* what);
 
 // ---------------------------------------------------------------------------
 // broadcast operand descriptor

@@ -29,6 +29,8 @@ int xg_check_launch(const char* what) {
   return XG_OK;
 }
 
+void xg_set_last_launch(const char* what) { g_last_launch = what; }
+
 extern "C" const char* xg_last_launch(void) { return g_last_launch; }
 
 extern "C" long long xg_launch_count(void) { return g_launches.load(std::memory_order_relaxed); }

@@ -14,6 +14,8 @@
 // stream touches (the per-slab halo planes, a scratch buffer); and the aux operands uploaded whole once per call.
 // Its mutex makes calls on one device take turns (they would fight for PCIe anyway); calls on different devices
 // run concurrently.  Streams and events live for the process; xg_host_workspace_release() frees the buffers.
+// A host device group (xg_host_group) spreads one call over several devices: spread() gives each member a block of
+// the result rows on its own thread, and each member streams its block through its own workspace.
 //
 // The stencil entry points here slab dim 0.  xg_stencil2_host: when dim 0 is the operated axis, consecutive slabs
 // overlap by the one-cell halo and the exterior halo plane (periodic wrap) is uploaded once.
@@ -25,6 +27,7 @@
 // folded row, for the fold).
 #include <stdlib.h>
 
+#include <thread>
 #include <vector>
 
 #include "xg_host.cuh"
@@ -154,6 +157,69 @@ int64_t slab_budget_bytes() {
   return target_bytes;
 }
 
+namespace {
+
+std::mutex g_group_mu;                  // guards g_groups
+std::vector<std::vector<int>> g_groups;  // member lists of the handles XG_HOST_GROUP_BASE + k; append-only
+
+// the member list of group handle `handle`; XG_EINVAL for an unknown handle (no CUDA call)
+int group_members(const char* who, int handle, std::vector<int>* members) {
+  std::lock_guard<std::mutex> lock(g_group_mu);
+  const int64_t k = (int64_t)handle - XG_HOST_GROUP_BASE;
+  if (k < 0 || k >= (int64_t)g_groups.size())
+    return xg_fail(XG_EINVAL, std::string(who) + ": unknown host device group " + std::to_string(handle));
+  *members = g_groups[(size_t)k];
+  return XG_OK;
+}
+
+}  // namespace
+
+int spread(const char* who, int device, int64_t L, bool edge_pairs, const BlockFn& body, bool split) {
+  if (device < XG_HOST_GROUP_BASE) return body(device, 0, L);
+  std::vector<int> members;
+  int rc = group_members(who, device, &members);
+  if (rc) return rc;
+  int64_t nb = split ? (int64_t)members.size() : 1;
+  if (nb > L) nb = L;
+  if (edge_pairs)  // the last block, the smallest, holds L / nb rows
+    while (nb > 1 && L / nb < 2) --nb;
+  if (nb < 1) nb = 1;
+  struct Outcome {
+    int rc = XG_OK;
+    std::string error;
+    const char* label = "";
+  };
+  std::vector<Outcome> res((size_t)nb);
+  std::vector<std::thread> threads;
+  threads.reserve((size_t)nb);
+  for (int64_t k = 0; k < nb; ++k) {
+    // the first L % nb blocks hold one row more
+    const int64_t r0 = k * (L / nb) + (k < L % nb ? k : L % nb), r1 = r0 + L / nb + (k < L % nb ? 1 : 0);
+    Outcome& o = res[(size_t)k];
+    const int member = members[(size_t)k];
+    try {
+      threads.emplace_back([&body, &o, member, r0, r1] {
+        try {
+          o.rc = body(member, r0, r1);
+        } catch (const std::exception& e) {
+          o.rc = xg_fail(XG_ECUDA, std::string("host device group member: ") + e.what());
+        }
+        if (o.rc) o.error = xg_last_error();
+        o.label = xg_last_launch();
+      });
+    } catch (const std::exception& e) {  // blocks k.. do not run
+      o.rc = XG_ECUDA;
+      o.error = std::string(who) + ": cannot start a thread for a host device group member: " + e.what();
+      break;
+    }
+  }
+  for (std::thread& t : threads) t.join();
+  xg_set_last_launch(res[0].label);
+  for (const Outcome& o : res)
+    if (o.rc) return xg_fail(o.rc, o.error);
+  return XG_OK;
+}
+
 Session::~Session() {
   if (w_ && w_->ready)
     for (cudaStream_t st : {w_->s_h2d, w_->s_k, w_->s_d2h}) cudaStreamSynchronize(st);
@@ -217,10 +283,11 @@ int Session::download(void* host, const void* dev, size_t bytes) {
 int Session::run(size_t es, const void* hin, const View3& in, int nout, void* const* hout, const View3* out,
                  const LaunchFn& launch, const PipeExtra& ex) {
   Workspace* w = w_;
-  const int64_t L = out[0].L;
-  if (in.L == 0 || in.C == 0 || in.R == 0 || L == 0) return XG_OK;
-  const int64_t rows = slab_rows(L, ex.row_bytes > 0 ? ex.row_bytes : in.C * in.R * (int64_t)es, ex.edge_pairs);
-  const int64_t nslab = xg_ceil_div(L, rows);
+  const int64_t r0 = ex.r0, r1 = ex.r1 < 0 ? out[0].L : ex.r1;
+  if (in.L == 0 || in.C == 0 || in.R == 0 || r1 <= r0) return XG_OK;
+  const int64_t rows =
+      slab_rows(r1 - r0, ex.row_bytes > 0 ? ex.row_bytes : in.C * in.R * (int64_t)es, ex.edge_pairs);
+  const int64_t nslab = xg_ceil_div(r1 - r0, rows);
   int rc = XG_OK;
   for (int i = 0; rc == XG_OK && i < kSlots; ++i) {
     rc = ensure(w->in[i], (size_t)(in.C * (rows + ex.lo_rows + ex.hi_rows) * in.R) * es);
@@ -236,7 +303,7 @@ int Session::run(size_t es, const void* hin, const View3& in, int nout, void* co
   int64_t p0 = 0, p1 = 0;                 // input rows the previous slab's buffer holds
   for (int64_t s = 0; s < nslab; ++s) {
     const int slot = (int)(s % kSlots);
-    const int64_t j0 = s * rows, j1 = (j0 + rows < L) ? j0 + rows : L;
+    const int64_t j0 = r0 + s * rows, j1 = (j0 + rows < r1) ? j0 + rows : r1;
     const int64_t i0 = (j0 - ex.lo_rows < 0) ? 0 : j0 - ex.lo_rows;
     const int64_t i1 = (j1 + ex.hi_rows > in.L) ? in.L : j1 + ex.hi_rows;
     if (s >= kSlots) {
@@ -244,7 +311,8 @@ int Session::run(size_t es, const void* hin, const View3& in, int nout, void* co
       XG_CUDA(cudaStreamWaitEvent(w->s_k, w->e_down[slot], 0));    // downloads out of this slot's results
     }
     char* d_in = static_cast<char*>(w->in[slot].p);
-    const int64_t keep = (s > 0 && p1 > i0) ? p1 - i0 : 0;  // rows [i0, i0 + keep) are on the device already
+    // rows [i0, i0 + keep) are on the device already (never in a block's first slab: its halo rows come up too)
+    const int64_t keep = (s > 0 && p1 > i0) ? p1 - i0 : 0;
     if (keep)  // same in-order stream as the uploads
       rc = copy_rows(d_in, (size_t)(i1 - i0) * row,
                      static_cast<const char*>(w->in[(s - 1) % kSlots].p) + (size_t)(i0 - p0) * row,
@@ -281,6 +349,8 @@ namespace {
 int workspace_bytes(const char* who, int device, int64_t* bytes) {
   if (!bytes) return xg_fail(XG_EINVAL, std::string(who) + ": null pointer");
   *bytes = 0;
+  if (device >= XG_HOST_GROUP_BASE)
+    return xg_fail(XG_EINVAL, std::string(who) + ": takes a device index, not a host device group");
   Workspace* w = nullptr;
   {
     std::lock_guard<std::mutex> reg(g_registry);
@@ -396,16 +466,18 @@ int validate_pair_call(const char* who, const Call& c, const PairTerm& t) {
 }
 
 // A slab's halo stage, on the kernel stream before its stencil launch: builds the slab's halo planes into b.plane
-// and points *hl / *hh at them.  `slab_shape` is the slab's shape, `pre` its rows of the pre-metric.
-typedef std::function<int(const SlabBufs& b, const int64_t* slab_shape, const void* pre, cudaStream_t st,
-                          const void** hl, const void** hh)>
+// and points *hl / *hh at them.  `slab_shape` is the slab's shape, `pre` its rows of the pre-metric, `fill` the
+// device copy of the fill constant (nullptr unless the entry point uploads one).  Called from every thread of a
+// host device group at once: it keeps no state across calls.
+typedef std::function<int(const SlabBufs& b, const int64_t* slab_shape, const void* pre, const void* fill,
+                          cudaStream_t st, const void** hl, const void** hh)>
     HaloFn;
 
 // The fold's halo stage: the folded north row of the slab (of the field across the fold: the input, or the second
 // input of a pair) is halo_hi, and halo_lo too when the south edge is periodic (it wraps the row above the top).
 HaloFn fold_stage(const Call& c, bool of_in2, int seam_axis, int skip, int64_t mirror, int64_t period, int negate) {
-  return [=](const SlabBufs& b, const int64_t* slab_shape, const void* pre, cudaStream_t st, const void** hl,
-             const void** hh) {
+  return [=](const SlabBufs& b, const int64_t* slab_shape, const void* pre, const void*, cudaStream_t st,
+             const void** hl, const void** hh) {
     *hh = b.plane[1];
     if (c.lo && c.bc == XG_BC_PERIODIC) *hl = *hh;
     return xg_fold_rows(c.dtype, of_in2 ? b.in2 : b.in, b.plane[1], c.ndim, slab_shape, c.axis, seam_axis, 1, 0, 1,
@@ -413,11 +485,12 @@ HaloFn fold_stage(const Call& c, bool of_in2, int seam_axis, int skip, int64_t m
   };
 }
 
-// A stencil entry point on the open session: field c.in in slabs along dim 0, `partner` (field b of pair `t`, or the
-// partner vector component, `partner_row` elements per dim-0 index) beside it, the metrics uploaded whole.  Per slab
-// `halo` (when dim 0 is a batch dim) builds the halo planes, then one xg_stencil2 or xg_stencil_pair_halo launch.
-int stencil_host(Session& ss, const Call& c, const PairTerm* t, const void* partner, int64_t partner_row,
-                 const HaloFn& halo) {
+// A stencil entry point (arguments checked) on c.device: field c.in in slabs along dim 0, `partner` (field b of pair
+// `t`, or the partner vector component, `partner_row` elements per dim-0 index) beside it, the metrics (and the
+// `fill_host` constant, es bytes, when given) uploaded whole.  Per slab `halo` (when dim 0 is a batch dim) builds
+// the halo planes, then one xg_stencil2 or xg_stencil_pair_halo launch.
+int stencil_host(const char* who, const Call& c, const PairTerm* t, const void* partner, int64_t partner_row,
+                 const HaloFn& halo, const void* fill_host = nullptr) {
   const size_t es = c.dtype == XG_F32 ? 4 : 8;
   const int ndim = c.ndim, lo = c.lo;
   const bool ax0 = c.axis == 0;
@@ -426,59 +499,67 @@ int stencil_host(Session& ss, const Call& c, const PairTerm* t, const void* part
   for (int d = 0; d < ndim; ++d) out_shape[d] = c.shape[d];
   out_shape[c.axis] = c.shape[c.axis] + c.lo + c.hi - 1;
   const View3 vin = view3(ndim, c.shape, 0), vout = view3(ndim, out_shape, 0);
-  if (vout.L <= 0 || vout.R == 0 || vin.R == 0) return XG_OK;
+  const bool edge_pairs = ax0 && c.bc == XG_BC_EXTRAPOLATE && (lo || c.hi);
+  return spread(who, c.device, vout.L, edge_pairs, [&](int device, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(device);
+    if (rc) return rc;
+    if (vout.L <= 0 || vout.R == 0 || vin.R == 0) return XG_OK;
 
-  const void *d_pre, *d_post, *d_pre_a = nullptr;
-  const void* wrap[2] = {nullptr, nullptr};  // periodic halo planes along dim 0: plane n0 - 1 below, plane 0 above
-  const size_t plane = (size_t)vin.R * es;
-  int rc = ss.upload(kAuxPre, c.pre, c.pre ? operand_span(c.pre_strides, c.shape, ndim, es) : 0, &d_pre);
-  if (rc == XG_OK)
-    rc = ss.upload(kAuxPost, c.post, c.post ? operand_span(c.post_strides, out_shape, ndim, es) : 0, &d_post);
-  if (rc == XG_OK && t && t->pre_a)
-    rc = ss.upload(kAuxPreA, t->pre_a, operand_span(t->pre_a_strides, c.shape, ndim, es), &d_pre_a);
-  if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && lo)
-    rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
-  if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && c.hi) rc = ss.upload(kAuxWrapHi, c.in, plane, &wrap[1]);
-  if (rc == XG_OK) rc = ss.fence();
-  if (rc) return rc;
+    const void *d_pre, *d_post, *d_pre_a = nullptr, *d_fill = nullptr;
+    const void* wrap[2] = {nullptr, nullptr};  // periodic halo planes along dim 0: plane n0 - 1 below, plane 0 above
+    const size_t plane = (size_t)vin.R * es;
+    rc = ss.upload(kAuxPre, c.pre, c.pre ? operand_span(c.pre_strides, c.shape, ndim, es) : 0, &d_pre);
+    if (rc == XG_OK)
+      rc = ss.upload(kAuxPost, c.post, c.post ? operand_span(c.post_strides, out_shape, ndim, es) : 0, &d_post);
+    if (rc == XG_OK && t && t->pre_a)
+      rc = ss.upload(kAuxPreA, t->pre_a, operand_span(t->pre_a_strides, c.shape, ndim, es), &d_pre_a);
+    if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && lo)
+      rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
+    if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && c.hi) rc = ss.upload(kAuxWrapHi, c.in, plane, &wrap[1]);
+    if (rc == XG_OK) rc = ss.upload(kAuxFill, fill_host, es, &d_fill);
+    if (rc == XG_OK) rc = ss.fence();
+    if (rc) return rc;
 
-  PipeExtra ex;
-  if (ax0) {  // result rows [j0, j1) read planes [j0 - lo, j1 - lo] of the padded field
-    ex.lo_rows = lo;
-    ex.hi_rows = 1 - lo;
-    ex.edge_pairs = c.bc == XG_BC_EXTRAPOLATE && (lo || c.hi);
-  }
-  if (partner) {
-    ex.hin2 = partner;
-    ex.in2 = View3{1, n0, partner_row};
-  }
-  if (halo) ex.plane_row_bytes = (size_t)(vin.R / c.shape[c.axis]) * es;
-  int64_t sshape[XG_MAX_NDIM];
-  for (int d = 0; d < ndim; ++d) sshape[d] = c.shape[d];
-  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
-    sshape[0] = i1 - i0;
-    const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(i0 * c.pre_strides[0]) * es : nullptr;
-    const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * c.post_strides[0]) * es : nullptr;
-    // along dim 0 a slab pads only the edges of the field its planes reach
-    const int slo = ax0 ? j0 - lo < 0 : lo, shi = ax0 ? j1 - lo + 1 > n0 : c.hi;
-    const void* hl = slo ? wrap[0] : nullptr;
-    const void* hh = shi ? wrap[1] : nullptr;
-    if (halo) {
-      const int rc2 = halo(b, sshape, pm, st, &hl, &hh);
-      if (rc2) return rc2;
+    PipeExtra ex;
+    if (ax0) {  // result rows [j0, j1) read planes [j0 - lo, j1 - lo] of the padded field
+      ex.lo_rows = lo;
+      ex.hi_rows = 1 - lo;
+      ex.edge_pairs = edge_pairs;
     }
-    if (t) {
-      const char* am = d_pre_a ? static_cast<const char*>(d_pre_a) + (size_t)(i0 * t->pre_a_strides[0]) * es : nullptr;
-      return xg_stencil_pair_halo(c.dtype, b.in, b.in2, b.out[0], ndim, sshape, t->op_a, t->lo_a, t->hi_a, t->bc_a,
-                                  t->fill_a, am, t->pre_a_strides, c.axis, c.op, lo, c.hi, c.bc, c.fill_value, pm,
-                                  c.pre_strides, t->subtract, qm, c.post_strides, hl, hh, st);
+    if (partner) {
+      ex.hin2 = partner;
+      ex.in2 = View3{1, n0, partner_row};
     }
-    return xg_stencil2(c.op, c.dtype, b.in, b.out[0], ndim, sshape, c.axis, slo, shi,
-                       (slo || shi) ? c.bc : XG_BC_NONE, c.fill_value, pm, c.pre_strides, qm, c.post_strides, hl, hh,
-                       st);
-  };
-  void* outs[1] = {c.out};
-  return ss.run(es, c.in, vin, 1, outs, &vout, launch, ex);
+    if (halo) ex.plane_row_bytes = (size_t)(vin.R / c.shape[c.axis]) * es;
+    int64_t sshape[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) sshape[d] = c.shape[d];
+    auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
+      sshape[0] = i1 - i0;
+      const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(i0 * c.pre_strides[0]) * es : nullptr;
+      const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * c.post_strides[0]) * es : nullptr;
+      // along dim 0 a slab pads only the edges of the field its planes reach
+      const int slo = ax0 ? j0 - lo < 0 : lo, shi = ax0 ? j1 - lo + 1 > n0 : c.hi;
+      const void* hl = slo ? wrap[0] : nullptr;
+      const void* hh = shi ? wrap[1] : nullptr;
+      if (halo) {
+        const int rc2 = halo(b, sshape, pm, d_fill, st, &hl, &hh);
+        if (rc2) return rc2;
+      }
+      if (t) {
+        const char* am =
+            d_pre_a ? static_cast<const char*>(d_pre_a) + (size_t)(i0 * t->pre_a_strides[0]) * es : nullptr;
+        return xg_stencil_pair_halo(c.dtype, b.in, b.in2, b.out[0], ndim, sshape, t->op_a, t->lo_a, t->hi_a, t->bc_a,
+                                    t->fill_a, am, t->pre_a_strides, c.axis, c.op, lo, c.hi, c.bc, c.fill_value, pm,
+                                    c.pre_strides, t->subtract, qm, c.post_strides, hl, hh, st);
+      }
+      return xg_stencil2(c.op, c.dtype, b.in, b.out[0], ndim, sshape, c.axis, slo, shi,
+                         (slo || shi) ? c.bc : XG_BC_NONE, c.fill_value, pm, c.pre_strides, qm, c.post_strides, hl, hh,
+                         st);
+    };
+    void* outs[1] = {c.out};
+    return ss.run(es, c.in, vin, 1, outs, &vout, launch, ex.rows(r0, r1));
+  });
 }
 
 // lowest and highest element a strided copy of `shape` touches from `offset`
@@ -510,6 +591,33 @@ extern "C" int xg_host_workspace_release(void) {
   return XG_OK;
 }
 
+extern "C" int xg_host_group(int n, const int* devices, int* group) {
+  const std::string who = "xg_host_group";
+  if (!devices || !group) return xg_fail(XG_EINVAL, who + ": null pointer");
+  if (n < 1 || n > XG_HOST_GROUP_MAX_MEMBERS)
+    return xg_fail(XG_EINVAL, who + ": between 1 and " + std::to_string(XG_HOST_GROUP_MAX_MEMBERS) + " members");
+  for (int k = 0; k < n; ++k)
+    if (devices[k] < 0) return xg_fail(XG_EINVAL, who + ": negative device index");
+  int count = 0;
+  XG_CUDA(cudaGetDeviceCount(&count));
+  for (int k = 0; k < n; ++k)
+    if (devices[k] >= count)
+      return xg_fail(XG_EINVAL, who + ": device " + std::to_string(devices[k]) + " does not exist (" +
+                                    std::to_string(count) + " visible)");
+  const std::vector<int> members(devices, devices + n);
+  std::lock_guard<std::mutex> lock(g_group_mu);
+  for (size_t k = 0; k < g_groups.size(); ++k)
+    if (g_groups[k] == members) {
+      *group = XG_HOST_GROUP_BASE + (int)k;
+      return XG_OK;
+    }
+  if (g_groups.size() >= XG_HOST_GROUP_MAX)
+    return xg_fail(XG_EINVAL, who + ": " + std::to_string(XG_HOST_GROUP_MAX) + " groups are registered already");
+  g_groups.push_back(members);
+  *group = XG_HOST_GROUP_BASE + (int)(g_groups.size() - 1);
+  return XG_OK;
+}
+
 extern "C" int xg_host_workspace_bytes(int device, int64_t* bytes) {
   return workspace_bytes("xg_host_workspace_bytes", device, bytes);
 }
@@ -526,10 +634,7 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
   const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, bc, fill_value,
                pre_metric, pre_strides, post_metric, post_strides, device};
   int rc = validate_call("xg_stencil2_host", c);
-  if (rc) return rc;
-  Session ss;
-  rc = ss.open(device);
-  return rc ? rc : stencil_host(ss, c, nullptr, nullptr, 0, nullptr);
+  return rc ? rc : stencil_host("xg_stencil2_host", c, nullptr, nullptr, 0, nullptr);
 }
 
 extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
@@ -542,10 +647,8 @@ extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* ou
                pre_metric, pre_strides, post_metric, post_strides, device};
   int rc = validate_halo_call(who, c);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
-  if (rc) return rc;
-  Session ss;
-  rc = ss.open(device);
-  return rc ? rc : stencil_host(ss, c, nullptr, nullptr, 0, fold_stage(c, false, seam_axis, skip, mirror, period, negate));
+  return rc ? rc
+            : stencil_host(who, c, nullptr, nullptr, 0, fold_stage(c, false, seam_axis, skip, mirror, period, negate));
 }
 
 extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, const void* partner,
@@ -619,21 +722,18 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   if ((lo && covered[0] != n0 * plane_row) || (hi && covered[1] != n0 * plane_row))
     return xg_fail(XG_EINVAL, who + ": the copies do not cover the halo planes");
 
-  Session ss;
-  rc = ss.open(device);
-  if (rc) return rc;
   const size_t es = dtype == XG_F32 ? 4 : 8;
-  const void* d_fill = nullptr;
   const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
-  if (fill) rc = ss.upload(kAuxFill, es == 4 ? (const void*)&f32 : (const void*)&fill_value, es, &d_fill);
-  if (rc) return rc;
-  // the whole-field copy list rebased onto each slab's buffers, `rows` high
-  std::vector<void*> dptr(ncopies);
-  std::vector<const void*> sptr(ncopies);
-  std::vector<int64_t> shp(shapes ? shapes : (const int64_t*)nullptr,
-                           shapes ? shapes + (size_t)ncopies * copy_ndim : (const int64_t*)nullptr);
-  auto copies = [&](const SlabBufs& b, const int64_t* slab_shape, const void*, cudaStream_t st, const void** hl,
-                    const void** hh) -> int {
+  const void* fill_host = fill ? (es == 4 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
+  // the whole-field copy list rebased onto each slab's buffers, `rows` high.  The rebased pointers and shapes are
+  // built per slab, on every path (three vectors of ncopies entries, small beside a slab's copies): the stage then
+  // keeps no state between slabs, so the members of a host device group can run it at once.
+  auto copies = [&](const SlabBufs& b, const int64_t* slab_shape, const void*, const void* d_fill, cudaStream_t st,
+                    const void** hl, const void** hh) -> int {
+    std::vector<void*> dptr(ncopies);
+    std::vector<const void*> sptr(ncopies);
+    std::vector<int64_t> shp(shapes ? shapes : (const int64_t*)nullptr,
+                             shapes ? shapes + (size_t)ncopies * copy_ndim : (const int64_t*)nullptr);
     for (int k = 0; k < ncopies; ++k) {
       dptr[k] = static_cast<char*>(b.plane[side[k]]) + (size_t)dst_offset[k] * es;
       const void* base = source[k] == kSrcField ? b.in : source[k] == kSrcPartner ? b.in2 : d_fill;
@@ -653,7 +753,7 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
     }
     return XG_OK;
   };
-  return stencil_host(ss, c, nullptr, partner, partner_row, copies);
+  return stencil_host(who.c_str(), c, nullptr, partner, partner_row, copies, fill_host);
 }
 
 extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,
@@ -665,10 +765,7 @@ extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, voi
   const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
                pre_b, pre_b_strides, post, post_strides, device};
   int rc = validate_pair_call("xg_stencil_pair_host", c, t);
-  if (rc) return rc;
-  Session ss;
-  rc = ss.open(device);
-  return rc ? rc : stencil_host(ss, c, &t, b, view3(ndim, shape, 0).R, nullptr);
+  return rc ? rc : stencil_host("xg_stencil_pair_host", c, &t, b, view3(ndim, shape, 0).R, nullptr);
 }
 
 extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, void* out, int ndim,
@@ -684,10 +781,7 @@ extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b
                pre_b, pre_b_strides, post, post_strides, device};
   int rc = validate_pair_call(who, c, t);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
-  if (rc) return rc;
-  Session ss;
-  rc = ss.open(device);
   return rc ? rc
-            : stencil_host(ss, c, &t, b, view3(ndim, shape, 0).R,
+            : stencil_host(who, c, &t, b, view3(ndim, shape, 0).R,
                            fold_stage(c, true, seam_axis, skip, mirror, period, negate));
 }

@@ -1,7 +1,9 @@
 // The slab engine of the host-buffer entry points (defined in xg_host.cu): one workspace per device, one pipeline
 //     H2D(slab s+1)  ||  kernel(s)(slab s)  ||  D2H(slab s-1)
-// on three streams with three slots.  The entry points validate their arguments, open a Session, upload their
-// whole-call operands, and pass Session::run a [C][L][R] view of the field and a launch callback.
+// on three streams with three slots.  The entry points validate their arguments, then, through spread(), on each
+// device of the call (one, or the members of a host device group, each with its block of result rows): open a
+// Session, upload their whole-call operands, and pass Session::run a [C][L][R] view of the field, a launch callback
+// and the block.
 #pragma once
 
 #include <functional>
@@ -58,6 +60,16 @@ struct PipeExtra {
   size_t scratch_row_bytes = 0, plane_row_bytes = 0;
   // Bytes one slab row moves, which size the slabs (0: the first input's)
   int64_t row_bytes = 0;
+  // Result rows [r0, r1) of the slab dim that run streams (r1 < 0: to the end); the slabs are sized within them,
+  // while row indices, halo rows and field edges stay those of the whole field
+  int64_t r0 = 0, r1 = -1;
+
+  PipeExtra rows(int64_t a, int64_t b) const {
+    PipeExtra e = *this;
+    e.r0 = a;
+    e.r1 = b;
+    return e;
+  }
 };
 
 struct Workspace;
@@ -91,5 +103,16 @@ class Session {
 size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size_t es);
 
 int64_t slab_budget_bytes();  // XG_HOST_SLAB_MB, default 128 MiB
+
+// body(device, r0, r1): one device's share of a host call, result rows [r0, r1) of the slab dim (extent L)
+typedef std::function<int(int, int64_t, int64_t)> BlockFn;
+
+// Run a host call on `device`: a device index, or a handle of xg_host_group.  A device index runs body(device, 0, L)
+// on the calling thread.  A group cuts [0, L) into contiguous near-equal blocks, at most one per member (one when
+// `split` is false), with no one-row block at a field edge under `edge_pairs`, and runs body(member, r0, r1) on
+// one thread per block; every thread is joined, error or not.  Returns the first failing block's status, with its
+// xg_last_error() text, and leaves the first block's xg_last_launch() label on the calling thread.  An unknown
+// handle gives XG_EINVAL before any CUDA call.
+int spread(const char* who, int device, int64_t L, bool edge_pairs, const BlockFn& body, bool split = true);
 
 }  // namespace xg_host

@@ -145,11 +145,10 @@ int check_theta(const char* fn, int ndim, const int64_t* tshape, const int64_t* 
   return XG_OK;
 }
 
-// Build the plan once the session is open; theta holds `tn` values along the axis (n + 1 bounds, n centres, or the
-// n levels of the linear twin).  A broadcast theta goes up whole (kAuxTheta); plan_theta_bounds makes the bounds
-// of one that holds centres.
-int plan_theta(Session& ss, ThetaPlan* p, int dtype, const void* theta, const int64_t* strides, int centers,
-               int64_t tn, int ndim, const int64_t* shape, int axis) {
+// The plan, before any device is touched; theta holds `tn` values along the axis (n + 1 bounds, n centres, or the
+// n levels of the linear twin).
+void plan_theta(ThetaPlan* p, int dtype, const int64_t* strides, int centers, int64_t tn, int ndim,
+                const int64_t* shape, int axis) {
   p->dtype = dtype;
   p->es = dtype == XG_F32 ? 4 : 8;
   p->ndim = ndim;
@@ -159,10 +158,15 @@ int plan_theta(Session& ss, ThetaPlan* p, int dtype, const void* theta, const in
   p->tshape[axis] = tn;
   p->bshape[axis] = p->centers ? tn + 1 : tn;
   p->dense = is_dense(ndim, p->tshape, strides);
+}
+
+// On the open session: a broadcast theta goes up whole (kAuxTheta); plan_theta_bounds makes the bounds of one that
+// holds centres.
+int upload_theta(Session& ss, ThetaPlan* p, const void* theta, const int64_t* strides) {
   if (p->dense) return XG_OK;
-  int rc = ss.upload(kAuxTheta, theta, operand_span(strides, p->tshape, ndim, p->es), &p->d_bcast);
+  int rc = ss.upload(kAuxTheta, theta, operand_span(strides, p->tshape, p->ndim, p->es), &p->d_bcast);
   if (rc) return rc;
-  for (int d = 0; d < ndim; ++d) p->bstrides[d] = strides[d];
+  for (int d = 0; d < p->ndim; ++d) p->bstrides[d] = strides[d];
   return XG_OK;
 }
 
@@ -260,64 +264,67 @@ extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const 
       if (hi[k] > ex.hi_rows) ex.hi_rows = hi[k];
     }
   }
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
-
-  const View3 vin = view3(ndim, shape, 0);
-  View3 vout[kMaxOut];
-  int64_t out_shape[kMaxOut][XG_MAX_NDIM];
-  for (int k = 0; k < nout; ++k) {
-    for (int d = 0; d < ndim; ++d) out_shape[k][d] = shape[d];
-    out_shape[k][axis[k]] = shape[axis[k]] + lo[k] + hi[k] - 1;
-    vout[k] = view3(ndim, out_shape[k], 0);
-    if (vout[k].R == 0 || vout[k].L == 0) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: empty result");
-  }
-  const int64_t n0 = shape[0];
-  // periodic wrap planes for results operated along dim 0: plane n0-1 below the first slab, plane 0 above the last
-  const void* d_wrap[2] = {nullptr, nullptr};
-  bool need_wrap = false;
-  for (int k = 0; k < nout; ++k) need_wrap = need_wrap || (axis[k] == 0 && bc[k] == XG_BC_PERIODIC);
-  if (need_wrap) {
-    const size_t pb = (size_t)vin.R * es;
-    rc = ss.upload(kAuxWrapLo, static_cast<const char*>(in) + (size_t)(n0 - 1) * pb, pb, &d_wrap[0]);
-    if (rc == XG_OK) rc = ss.upload(kAuxWrapHi, in, pb, &d_wrap[1]);
-    if (rc == XG_OK) rc = ss.fence();
+  // every result keeps the extent of dim 0, the slab dim
+  return spread("xg_stencil2_host_multi", device, shape[0], false, [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
     if (rc) return rc;
-  }
-  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+
+    const View3 vin = view3(ndim, shape, 0);
+    View3 vout[kMaxOut];
+    int64_t out_shape[kMaxOut][XG_MAX_NDIM];
     for (int k = 0; k < nout; ++k) {
-      const char* src = static_cast<const char*>(b.in);
-      int slo = lo[k], shi = hi[k], sbc = bc[k];
-      const void* hl = nullptr;
-      const void* hh = nullptr;
-      if (axis[k] == 0) {
-        // output rows [j0, j1) need P[j0 .. j1], i.e. source planes [j0 - lo, j1 - lo] clipped to the field
-        int64_t s0 = j0 - lo[k], s1 = j1 - lo[k] + 1;
-        slo = shi = 0;
-        if (s0 < 0) { s0 = 0; slo = 1; }
-        if (s1 > n0) { s1 = n0; shi = 1; }
-        if (s0 < i0 || s1 > i1) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: internal slab window error");
-        src += (size_t)(s0 - i0) * vin.R * es;
-        sshape[0] = s1 - s0;
-        if (bc[k] == XG_BC_PERIODIC) {
-          if (slo) hl = d_wrap[0];
-          if (shi) hh = d_wrap[1];
-        }
-        if (!slo && !shi) sbc = XG_BC_NONE;
-      } else {
-        src += (size_t)(j0 - i0) * vin.R * es;
-        sshape[0] = j1 - j0;
-      }
-      const int rc2 = xg_stencil2(op[k], dtype, src, b.out[k], ndim, sshape, axis[k], slo, shi, sbc, fill_value[k],
-                                  nullptr, nullptr, nullptr, nullptr, hl, hh, st);
-      if (rc2) return rc2;
+      for (int d = 0; d < ndim; ++d) out_shape[k][d] = shape[d];
+      out_shape[k][axis[k]] = shape[axis[k]] + lo[k] + hi[k] - 1;
+      vout[k] = view3(ndim, out_shape[k], 0);
+      if (vout[k].R == 0 || vout[k].L == 0) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: empty result");
     }
-    return XG_OK;
-  };
-  return ss.run(es, in, vin, nout, out, vout, launch, ex);
+    const int64_t n0 = shape[0];
+    // periodic wrap planes for results operated along dim 0: plane n0-1 below the first slab, plane 0 above the last
+    const void* d_wrap[2] = {nullptr, nullptr};
+    bool need_wrap = false;
+    for (int k = 0; k < nout; ++k) need_wrap = need_wrap || (axis[k] == 0 && bc[k] == XG_BC_PERIODIC);
+    if (need_wrap) {
+      const size_t pb = (size_t)vin.R * es;
+      rc = ss.upload(kAuxWrapLo, static_cast<const char*>(in) + (size_t)(n0 - 1) * pb, pb, &d_wrap[0]);
+      if (rc == XG_OK) rc = ss.upload(kAuxWrapHi, in, pb, &d_wrap[1]);
+      if (rc == XG_OK) rc = ss.fence();
+      if (rc) return rc;
+    }
+    auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      for (int k = 0; k < nout; ++k) {
+        const char* src = static_cast<const char*>(b.in);
+        int slo = lo[k], shi = hi[k], sbc = bc[k];
+        const void* hl = nullptr;
+        const void* hh = nullptr;
+        if (axis[k] == 0) {
+          // output rows [j0, j1) need P[j0 .. j1], i.e. source planes [j0 - lo, j1 - lo] clipped to the field
+          int64_t s0 = j0 - lo[k], s1 = j1 - lo[k] + 1;
+          slo = shi = 0;
+          if (s0 < 0) { s0 = 0; slo = 1; }
+          if (s1 > n0) { s1 = n0; shi = 1; }
+          if (s0 < i0 || s1 > i1) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: internal slab window error");
+          src += (size_t)(s0 - i0) * vin.R * es;
+          sshape[0] = s1 - s0;
+          if (bc[k] == XG_BC_PERIODIC) {
+            if (slo) hl = d_wrap[0];
+            if (shi) hh = d_wrap[1];
+          }
+          if (!slo && !shi) sbc = XG_BC_NONE;
+        } else {
+          src += (size_t)(j0 - i0) * vin.R * es;
+          sshape[0] = j1 - j0;
+        }
+        const int rc2 = xg_stencil2(op[k], dtype, src, b.out[k], ndim, sshape, axis[k], slo, shi, sbc, fill_value[k],
+                                    nullptr, nullptr, nullptr, nullptr, hl, hh, st);
+        if (rc2) return rc2;
+      }
+      return XG_OK;
+    };
+    return ss.run(es, in, vin, nout, out, vout, launch, ex.rows(r0, r1));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -385,37 +392,39 @@ extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int n
   const size_t es = dtype == XG_F32 ? 4 : 8;
   const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
   ex.row_bytes = (vin.C * vin.R + vout.C * vout.R) * (int64_t)es;
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
-  const int64_t n = shape[sd];
-  auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM];
-    int slo[3], shi[3], sbc[3];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    for (int k = 0; k < naxes; ++k) {
-      slo[k] = lo[k];
-      shi[k] = hi[k];
-      sbc[k] = bc[k];
-    }
-    const char* src = static_cast<const char*>(b.in);
-    if (ka >= 0) {
-      // result rows [j0, j1) need padded planes [j0, j1], i.e. input rows [j0 - lo, j1 - lo] clipped to the field:
-      // an inner slab edge reads its neighbour row, the field's own ends keep the call's boundary condition
-      int64_t s0 = j0 - lo[ka], s1 = j1 - lo[ka] + 1;
-      slo[ka] = shi[ka] = 0;
-      if (s0 < 0) { s0 = 0; slo[ka] = 1; }
-      if (s1 > n) { s1 = n; shi[ka] = 1; }
-      if (s0 < i0 || s1 > i1 || vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
-      if (!slo[ka] && !shi[ka]) sbc[ka] = XG_BC_NONE;
-      src += (size_t)(s0 - i0) * vin.R * es;
-      sshape[sd] = s1 - s0;
-    } else {
-      sshape[sd] = j1 - j0;
-    }
-    return xg_stencil_multi(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc, fill_value, st);
-  };
-  return ss.run(es, in, vin, 1, &out, &vout, launch, ex);
+  return spread(who.c_str(), device, vout.L, false, [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
+    if (rc) return rc;
+    const int64_t n = shape[sd];
+    auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM];
+      int slo[3], shi[3], sbc[3];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      for (int k = 0; k < naxes; ++k) {
+        slo[k] = lo[k];
+        shi[k] = hi[k];
+        sbc[k] = bc[k];
+      }
+      const char* src = static_cast<const char*>(b.in);
+      if (ka >= 0) {
+        // result rows [j0, j1) need padded planes [j0, j1], i.e. input rows [j0 - lo, j1 - lo] clipped to the field:
+        // an inner slab edge reads its neighbour row, the field's own ends keep the call's boundary condition
+        int64_t s0 = j0 - lo[ka], s1 = j1 - lo[ka] + 1;
+        slo[ka] = shi[ka] = 0;
+        if (s0 < 0) { s0 = 0; slo[ka] = 1; }
+        if (s1 > n) { s1 = n; shi[ka] = 1; }
+        if (s0 < i0 || s1 > i1 || vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
+        if (!slo[ka] && !shi[ka]) sbc[ka] = XG_BC_NONE;
+        src += (size_t)(s0 - i0) * vin.R * es;
+        sshape[sd] = s1 - s0;
+      } else {
+        sshape[sd] = j1 - j0;
+      }
+      return xg_stencil_multi(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc, fill_value, st);
+    };
+    return ss.run(es, in, vin, 1, &out, &vout, launch, ex.rows(r0, r1));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -435,41 +444,44 @@ extern "C" int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, c
   int64_t out_shape[XG_MAX_NDIM];
   for (int d = 0; d < ndim; ++d) out_shape[d] = shape[d];
   out_shape[axis] = kept + pad_lo + pad_hi;
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
   const int sd = first_free_dim(ndim, axis);
-  const void* d_pre = nullptr;
-  const void* d_post = nullptr;
-  if (pre_metric) rc = ss.upload(kAuxPre, pre_metric, operand_span(pre_strides, shape, ndim, es), &d_pre);
-  if (rc) return rc;
-  if (post_metric) rc = ss.upload(kAuxPost, post_metric, operand_span(post_strides, out_shape, ndim, es), &d_post);
-  if (rc) return rc;
-  rc = ss.fence();
-  if (rc) return rc;
-  if (sd < 0) {  // 1-D: one slab = the whole line
-    const View3 v{1, 1, shape[0]}, vo{1, 1, out_shape[0]};
+  return spread("xg_cumscan_host", device, sd < 0 ? 1 : shape[sd], false,
+                [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
+    if (rc) return rc;
+    const void* d_pre = nullptr;
+    const void* d_post = nullptr;
+    if (pre_metric) rc = ss.upload(kAuxPre, pre_metric, operand_span(pre_strides, shape, ndim, es), &d_pre);
+    if (rc) return rc;
+    if (post_metric) rc = ss.upload(kAuxPost, post_metric, operand_span(post_strides, out_shape, ndim, es), &d_post);
+    if (rc) return rc;
+    rc = ss.fence();
+    if (rc) return rc;
+    if (sd < 0) {  // 1-D: one slab = the whole line
+      const View3 v{1, 1, shape[0]}, vo{1, 1, out_shape[0]};
+      void* outs[1] = {out};
+      auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+        return xg_cumscan(dtype, b.in, b.out[0], ndim, shape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value,
+                          d_pre, pre_strides, d_post, post_strides, skipna, st);
+      };
+      return ss.run(es, in, v, 1, outs, &vo, launch);
+    }
+    const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
     void* outs[1] = {out};
-    auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-      return xg_cumscan(dtype, b.in, b.out[0], ndim, shape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, d_pre,
-                        pre_strides, d_post, post_strides, skipna, st);
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      sshape[sd] = j1 - j0;
+      const char* pm = static_cast<const char*>(d_pre);
+      const char* qm = static_cast<const char*>(d_post);
+      if (pm) pm += (size_t)(j0 * pre_strides[sd]) * es;
+      if (qm) qm += (size_t)(j0 * post_strides[sd]) * es;
+      return xg_cumscan(dtype, b.in, b.out[0], ndim, sshape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, pm,
+                        pre_strides, qm, post_strides, skipna, st);
     };
-    return ss.run(es, in, v, 1, outs, &vo, launch);
-  }
-  const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
-  void* outs[1] = {out};
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    sshape[sd] = j1 - j0;
-    const char* pm = static_cast<const char*>(d_pre);
-    const char* qm = static_cast<const char*>(d_post);
-    if (pm) pm += (size_t)(j0 * pre_strides[sd]) * es;
-    if (qm) qm += (size_t)(j0 * post_strides[sd]) * es;
-    return xg_cumscan(dtype, b.in, b.out[0], ndim, sshape, axis, reverse, trim, pad_lo, pad_hi, bc, fill_value, pm,
-                      pre_strides, qm, post_strides, skipna, st);
-  };
-  return ss.run(es, in, vin, 1, outs, &vout, launch);
+    return ss.run(es, in, vin, 1, outs, &vout, launch, PipeExtra().rows(r0, r1));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -481,41 +493,44 @@ extern "C" int xg_wreduce_host(int dtype, const void* in, const void* weight, co
   if (axis < 0 || axis >= ndim) return xg_fail(XG_EINVAL, "xg_wreduce_host: axis out of range");
   if (weight && !w_strides) return xg_fail(XG_EINVAL, "xg_wreduce_host: weight strides missing");
   const size_t es = dtype == XG_F32 ? 4 : 8;
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
-  const void* d_w = nullptr;
-  if (weight) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
-  if (rc) return rc;
-  rc = ss.fence();
-  if (rc) return rc;
   const int sd = first_free_dim(ndim, axis);
-  void* outs[1] = {out};
-  if (sd < 0) {
-    const View3 v{1, 1, shape[0]}, vo{1, 1, 1};
-    auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-      return xg_wreduce(dtype, b.in, d_w, w_strides, b.out[0], ndim, shape, axis, mode, skipna, st);
+  return spread("xg_wreduce_host", device, sd < 0 ? 1 : shape[sd], false,
+                [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
+    if (rc) return rc;
+    const void* d_w = nullptr;
+    if (weight) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
+    if (rc) return rc;
+    rc = ss.fence();
+    if (rc) return rc;
+    void* outs[1] = {out};
+    if (sd < 0) {
+      const View3 v{1, 1, shape[0]}, vo{1, 1, 1};
+      auto launch = [&](int64_t, int64_t, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+        return xg_wreduce(dtype, b.in, d_w, w_strides, b.out[0], ndim, shape, axis, mode, skipna, st);
+      };
+      return ss.run(es, in, v, 1, outs, &vo, launch);
+    }
+    // result shape = shape without `axis`; the slab dim keeps its extent
+    int64_t out_shape[XG_MAX_NDIM];
+    int nd_o = 0, sd_o = 0;
+    for (int d = 0; d < ndim; ++d) {
+      if (d == axis) continue;
+      if (d == sd) sd_o = nd_o;
+      out_shape[nd_o++] = shape[d];
+    }
+    const View3 vin = view3(ndim, shape, sd), vout = view3(nd_o, out_shape, sd_o);
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      sshape[sd] = j1 - j0;
+      const char* wm = static_cast<const char*>(d_w);
+      if (wm) wm += (size_t)(j0 * w_strides[sd]) * es;
+      return xg_wreduce(dtype, b.in, wm, w_strides, b.out[0], ndim, sshape, axis, mode, skipna, st);
     };
-    return ss.run(es, in, v, 1, outs, &vo, launch);
-  }
-  // result shape = shape without `axis`; the slab dim keeps its extent
-  int64_t out_shape[XG_MAX_NDIM];
-  int nd_o = 0, sd_o = 0;
-  for (int d = 0; d < ndim; ++d) {
-    if (d == axis) continue;
-    if (d == sd) sd_o = nd_o;
-    out_shape[nd_o++] = shape[d];
-  }
-  const View3 vin = view3(ndim, shape, sd), vout = view3(nd_o, out_shape, sd_o);
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    sshape[sd] = j1 - j0;
-    const char* wm = static_cast<const char*>(d_w);
-    if (wm) wm += (size_t)(j0 * w_strides[sd]) * es;
-    return xg_wreduce(dtype, b.in, wm, w_strides, b.out[0], ndim, sshape, axis, mode, skipna, st);
-  };
-  return ss.run(es, in, vin, 1, outs, &vout, launch);
+    return ss.run(es, in, vin, 1, outs, &vout, launch, PipeExtra().rows(r0, r1));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -615,116 +630,119 @@ extern "C" int xg_wreduce_host_multi(int dtype, const void* in, const void* weig
   ex.row_bytes = (vin.C * vin.R + (stream_w ? ex.in2.C * ex.in2.R : 0) + scratch_el +
                   (whole ? 0 : vout.C * vout.R)) * (int64_t)es;
 
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
-  const void* d_w = nullptr;
-  if (weight && !stream_w) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
-  if (rc) return rc;
-  rc = ss.fence();
-  if (rc) return rc;
-  // `whole`: [sum partials (L)][valid-weight partials (L)], the results of the last launches, the mean
-  char* partial = nullptr;
-  int64_t partial_el = mult * L + 1;
-  if (whole) {
-    int64_t c[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) c[d] = shape[d];
-    int cn = ndim;
-    for (int k = 0; k < nord; ++k) {
-      for (int d = ord[k]; d + 1 < cn; ++d) c[d] = c[d + 1];
-      if (k >= nslab) partial_el += mult * numel(cn - 1, c);
-      --cn;
-    }
-    void* p = nullptr;
-    rc = ss.aux(kAuxPartial, (size_t)partial_el * es, &p);
+  // `whole` keeps its partials along the slab dim on one device: it runs on a group's first member alone
+  return spread(who.c_str(), device, L, false, [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
     if (rc) return rc;
-    partial = static_cast<char*>(p);
-  }
-  // launches k0 .. k1 - 1 of the chain on `cur` (cnd dims), from num_in (den_in: the valid weights of a mean), the
-  // weight with launch 0; the results of each go to the next free `scratch` elements, or to num_last / den_last
-  // for the last one when they are given
-  auto chain = [&](int k0, int k1, int64_t* cur, int cnd, const void* num_in, const void* den_in, const void* wp,
-                   const int64_t* ws, char* scratch, void* num_last, void* den_last, const void** num_out,
-                   const void** den_out, cudaStream_t st) -> int {
-    for (int k = k0; k < k1; ++k) {
-      const int64_t count = numel(cnd, cur) / cur[ord[k]];
-      void* nd = num_last;
-      void* dd = den_last;
-      if (k < k1 - 1 || !num_last) {
-        nd = scratch;
-        dd = mean ? scratch + (size_t)count * es : nullptr;
-        scratch += (size_t)(mult * count) * es;
-      }
-      int rc2;
-      if (k == 0) {
-        rc2 = mean ? xg_wreduce(dtype, num_in, wp, ws, dd, cnd, cur, ord[k], XG_REDUCE_WVALID, skipna, st) : XG_OK;
-        if (rc2 == XG_OK) rc2 = xg_wreduce(dtype, num_in, wp, ws, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
-      } else {
-        rc2 = xg_wreduce(dtype, num_in, nullptr, nullptr, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
-        if (rc2 == XG_OK && mean)
-          rc2 = xg_wreduce(dtype, den_in, nullptr, nullptr, dd, cnd, cur, ord[k], XG_REDUCE_SUM, 0, st);
-      }
-      if (rc2) return rc2;
-      num_in = nd;
-      den_in = dd;
-      for (int d = ord[k]; d + 1 < cnd; ++d) cur[d] = cur[d + 1];
-      --cnd;
-    }
-    *num_out = num_in;
-    *den_out = den_in;
-    return XG_OK;
-  };
-  // the mean: sum / valid weights, NaN where no weight is valid
-  auto divide = [&](const void* num, const void* den, void* res, int64_t count, cudaStream_t st) -> int {
-    const int64_t one = 1;
-    return xg_binary(XG_BIN_DIVNZ, dtype, num, den, &one, res, 1, &count, st);
-  };
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-    const int64_t rows = j1 - j0;
-    int64_t cur[XG_MAX_NDIM], ws[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) cur[d] = shape[d];
-    cur[sd] = rows;
-    const void* wp = nullptr;
-    if (stream_w) {  // the slab's own dense layout
+    const void* d_w = nullptr;
+    if (weight && !stream_w) rc = ss.upload(kAuxPre, weight, operand_span(w_strides, shape, ndim, es), &d_w);
+    if (rc) return rc;
+    rc = ss.fence();
+    if (rc) return rc;
+    // `whole`: [sum partials (L)][valid-weight partials (L)], the results of the last launches, the mean
+    char* partial = nullptr;
+    int64_t partial_el = mult * L + 1;
+    if (whole) {
       int64_t c[XG_MAX_NDIM];
-      for (int d = 0; d < ndim; ++d) c[d] = wshape[d];
-      c[sd] = rows;
-      dense_strides(ndim, c, ws);
-      for (int d = 0; d < ndim; ++d)
-        if (c[d] == 1) ws[d] = 0;
-      wp = b.in2;
-    } else if (d_w) {
-      for (int d = 0; d < ndim; ++d) ws[d] = w_strides[d];
-      wp = static_cast<const char*>(d_w) + (size_t)(j0 * w_strides[sd]) * es;
+      for (int d = 0; d < ndim; ++d) c[d] = shape[d];
+      int cn = ndim;
+      for (int k = 0; k < nord; ++k) {
+        for (int d = ord[k]; d + 1 < cn; ++d) c[d] = c[d + 1];
+        if (k >= nslab) partial_el += mult * numel(cn - 1, c);
+        --cn;
+      }
+      void* p = nullptr;
+      rc = ss.aux(kAuxPartial, (size_t)partial_el * es, &p);
+      if (rc) return rc;
+      partial = static_cast<char*>(p);
     }
-    void* num_last = whole ? partial + (size_t)j0 * es : (mean ? nullptr : b.out[0]);
-    void* den_last = whole && mean ? partial + (size_t)(L + j0) * es : nullptr;
-    const void *num, *den;
-    int rc2 = chain(0, nslab, cur, ndim, b.in, nullptr, wp, wp ? ws : nullptr, static_cast<char*>(b.scratch),
-                    num_last, den_last, &num, &den, st);
-    if (rc2 || whole || !mean) return rc2;
-    return divide(num, den, b.out[0], rows * rowel[nslab - 1], st);
-  };
-  if (!whole) return ss.run(es, in, vin, 1, &out, &vout, launch, ex);
-  rc = ss.run(es, in, vin, 0, nullptr, &vout, launch, ex);
-  if (rc) return rc;
-  // the launches along the slab dim and the dims in front of it, once, on the partials
-  int64_t cur[XG_MAX_NDIM];
-  int cnd = 0;
-  for (int d = 0; d < ndim; ++d)
-    if (!(red[d] && d > sd)) cur[cnd++] = shape[d];
-  const void *num, *den;
-  char* next = partial + (size_t)(mult * L) * es;
-  rc = chain(nslab, nord, cur, cnd, partial, mean ? partial + (size_t)L * es : nullptr, nullptr, nullptr, next,
-             nullptr, nullptr, &num, &den, ss.kernel_stream());
-  if (rc) return rc;
-  if (mean) {
-    void* res = partial + (size_t)(partial_el - 1) * es;  // the last element
-    rc = divide(num, den, res, 1, ss.kernel_stream());
+    // launches k0 .. k1 - 1 of the chain on `cur` (cnd dims), from num_in (den_in: the valid weights of a mean), the
+    // weight with launch 0; the results of each go to the next free `scratch` elements, or to num_last / den_last
+    // for the last one when they are given
+    auto chain = [&](int k0, int k1, int64_t* cur, int cnd, const void* num_in, const void* den_in, const void* wp,
+                     const int64_t* ws, char* scratch, void* num_last, void* den_last, const void** num_out,
+                     const void** den_out, cudaStream_t st) -> int {
+      for (int k = k0; k < k1; ++k) {
+        const int64_t count = numel(cnd, cur) / cur[ord[k]];
+        void* nd = num_last;
+        void* dd = den_last;
+        if (k < k1 - 1 || !num_last) {
+          nd = scratch;
+          dd = mean ? scratch + (size_t)count * es : nullptr;
+          scratch += (size_t)(mult * count) * es;
+        }
+        int rc2;
+        if (k == 0) {
+          rc2 = mean ? xg_wreduce(dtype, num_in, wp, ws, dd, cnd, cur, ord[k], XG_REDUCE_WVALID, skipna, st) : XG_OK;
+          if (rc2 == XG_OK) rc2 = xg_wreduce(dtype, num_in, wp, ws, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
+        } else {
+          rc2 = xg_wreduce(dtype, num_in, nullptr, nullptr, nd, cnd, cur, ord[k], XG_REDUCE_SUM, skipna, st);
+          if (rc2 == XG_OK && mean)
+            rc2 = xg_wreduce(dtype, den_in, nullptr, nullptr, dd, cnd, cur, ord[k], XG_REDUCE_SUM, 0, st);
+        }
+        if (rc2) return rc2;
+        num_in = nd;
+        den_in = dd;
+        for (int d = ord[k]; d + 1 < cnd; ++d) cur[d] = cur[d + 1];
+        --cnd;
+      }
+      *num_out = num_in;
+      *den_out = den_in;
+      return XG_OK;
+    };
+    // the mean: sum / valid weights, NaN where no weight is valid
+    auto divide = [&](const void* num, const void* den, void* res, int64_t count, cudaStream_t st) -> int {
+      const int64_t one = 1;
+      return xg_binary(XG_BIN_DIVNZ, dtype, num, den, &one, res, 1, &count, st);
+    };
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      const int64_t rows = j1 - j0;
+      int64_t cur[XG_MAX_NDIM], ws[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) cur[d] = shape[d];
+      cur[sd] = rows;
+      const void* wp = nullptr;
+      if (stream_w) {  // the slab's own dense layout
+        int64_t c[XG_MAX_NDIM];
+        for (int d = 0; d < ndim; ++d) c[d] = wshape[d];
+        c[sd] = rows;
+        dense_strides(ndim, c, ws);
+        for (int d = 0; d < ndim; ++d)
+          if (c[d] == 1) ws[d] = 0;
+        wp = b.in2;
+      } else if (d_w) {
+        for (int d = 0; d < ndim; ++d) ws[d] = w_strides[d];
+        wp = static_cast<const char*>(d_w) + (size_t)(j0 * w_strides[sd]) * es;
+      }
+      void* num_last = whole ? partial + (size_t)j0 * es : (mean ? nullptr : b.out[0]);
+      void* den_last = whole && mean ? partial + (size_t)(L + j0) * es : nullptr;
+      const void *num, *den;
+      int rc2 = chain(0, nslab, cur, ndim, b.in, nullptr, wp, wp ? ws : nullptr, static_cast<char*>(b.scratch),
+                      num_last, den_last, &num, &den, st);
+      if (rc2 || whole || !mean) return rc2;
+      return divide(num, den, b.out[0], rows * rowel[nslab - 1], st);
+    };
+    if (!whole) return ss.run(es, in, vin, 1, &out, &vout, launch, ex.rows(r0, r1));
+    rc = ss.run(es, in, vin, 0, nullptr, &vout, launch, ex);
     if (rc) return rc;
-    num = res;
-  }
-  return ss.download(out, num, es);
+    // the launches along the slab dim and the dims in front of it, once, on the partials
+    int64_t cur[XG_MAX_NDIM];
+    int cnd = 0;
+    for (int d = 0; d < ndim; ++d)
+      if (!(red[d] && d > sd)) cur[cnd++] = shape[d];
+    const void *num, *den;
+    char* next = partial + (size_t)(mult * L) * es;
+    rc = chain(nslab, nord, cur, cnd, partial, mean ? partial + (size_t)L * es : nullptr, nullptr, nullptr, next,
+               nullptr, nullptr, &num, &den, ss.kernel_stream());
+    if (rc) return rc;
+    if (mean) {
+      void* res = partial + (size_t)(partial_el - 1) * es;  // the last element
+      rc = divide(num, den, res, 1, ss.kernel_stream());
+      if (rc) return rc;
+      num = res;
+    }
+    return ss.download(out, num, es);
+  }, !whole);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -740,40 +758,45 @@ extern "C" int xg_vinterp_linear_host(int dtype, const void* phi, const void* th
   if (axis < 0 || axis >= ndim) return xg_fail(XG_EINVAL, "xg_vinterp_linear_host: axis out of range");
   if (m < 0) return xg_fail(XG_EINVAL, "xg_vinterp_linear_host: negative number of target levels");
   const size_t es = dtype == XG_F32 ? 4 : 8;
-  Session ss;
-  int rc = ss.open(device);
-  if (rc) return rc;
   // theta: a dense field streams beside phi, a broadcast one is uploaded whole; target whole
-  ThetaPlan tp;
-  rc = plan_theta(ss, &tp, dtype, theta, theta_strides, 0, shape[axis], ndim, shape, axis);
-  if (rc) return rc;
-  const void* d_target = nullptr;
-  int64_t tshape[XG_MAX_NDIM];
-  for (int d = 0; d < ndim; ++d) tshape[d] = shape[d];
-  tshape[axis] = m;
-  const size_t tbytes = target_strides ? operand_span(target_strides, tshape, ndim, es) : (size_t)m * es;
-  rc = ss.upload(kAuxTarget, target, tbytes ? tbytes : es, &d_target);
-  if (rc) return rc;
-  rc = ss.fence();
-  if (rc) return rc;
-  const TransformViews tv = transform_views(ndim, shape, axis, m, tp, theta);
-  tp.sd = tv.sd;
-  void* outs[1] = {out};
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    const char* tg = static_cast<const char*>(d_target);
-    if (tv.sd >= 0) {
-      sshape[tv.sd] = j1 - j0;
-      if (target_strides) tg += (size_t)(j0 * target_strides[tv.sd]) * es;
-    }
-    const void* th = nullptr;
-    const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
-    if (rc2) return rc2;
-    return xg_vinterp_linear(dtype, b.in, th, th_strides, tg, target_strides, m, b.out[0], ndim, sshape, axis,
-                             mask_edges, bypass_checks, logarithmic, st);
-  };
-  return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex);
+  ThetaPlan plan;
+  plan_theta(&plan, dtype, theta_strides, 0, shape[axis], ndim, shape, axis);
+  const TransformViews tv = transform_views(ndim, shape, axis, m, plan, theta);
+  plan.sd = tv.sd;
+  return spread("xg_vinterp_linear_host", device, tv.sd >= 0 ? shape[tv.sd] : 1, false,
+                [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
+    if (rc) return rc;
+    ThetaPlan tp = plan;
+    rc = upload_theta(ss, &tp, theta, theta_strides);
+    if (rc) return rc;
+    const void* d_target = nullptr;
+    int64_t tshape[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) tshape[d] = shape[d];
+    tshape[axis] = m;
+    const size_t tbytes = target_strides ? operand_span(target_strides, tshape, ndim, es) : (size_t)m * es;
+    rc = ss.upload(kAuxTarget, target, tbytes ? tbytes : es, &d_target);
+    if (rc) return rc;
+    rc = ss.fence();
+    if (rc) return rc;
+    void* outs[1] = {out};
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      const char* tg = static_cast<const char*>(d_target);
+      if (tv.sd >= 0) {
+        sshape[tv.sd] = j1 - j0;
+        if (target_strides) tg += (size_t)(j0 * target_strides[tv.sd]) * es;
+      }
+      const void* th = nullptr;
+      const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
+      if (rc2) return rc2;
+      return xg_vinterp_linear(dtype, b.in, th, th_strides, tg, target_strides, m, b.out[0], ndim, sshape, axis,
+                               mask_edges, bypass_checks, logarithmic, st);
+    };
+    return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex.rows(r0, r1));
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -810,32 +833,37 @@ extern "C" int xg_vinterp_conservative_host(int dtype, const void* phi, const vo
       for (int64_t i = 0; i < count; ++i) static_cast<double*>(out)[i] = NAN;
     return XG_OK;
   }
-  Session ss;
-  rc = ss.open(device);
-  if (rc) return rc;
   // theta: streamed (dense) or whole (its bounds made on the device at centres); bins whole
-  ThetaPlan tp;
-  rc = plan_theta(ss, &tp, dtype, theta, theta_strides, theta_at_centers, tshape[axis], ndim, shape, axis);
-  if (rc) return rc;
-  const void* d_bins = nullptr;
-  rc = ss.upload(kAuxTarget, target_bins, (size_t)m * es, &d_bins);
-  if (rc) return rc;
-  rc = ss.fence();
-  if (rc) return rc;
-  rc = plan_theta_bounds(ss, &tp, theta_strides);
-  if (rc) return rc;
-  const TransformViews tv = transform_views(ndim, shape, axis, m - 1, tp, theta);
-  tp.sd = tv.sd;
-  void* outs[1] = {out};
-  auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
-    int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-    if (tv.sd >= 0) sshape[tv.sd] = j1 - j0;
-    const void* th = nullptr;
-    const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
-    if (rc2) return rc2;
-    return xg_vinterp_conservative(dtype, b.in, th, th_strides, d_bins, m, flip_out, b.out[0], ndim, sshape, axis,
-                                   st);
-  };
-  return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex);
+  ThetaPlan plan;
+  plan_theta(&plan, dtype, theta_strides, theta_at_centers, tshape[axis], ndim, shape, axis);
+  const TransformViews tv = transform_views(ndim, shape, axis, m - 1, plan, theta);
+  plan.sd = tv.sd;
+  return spread("xg_vinterp_conservative_host", device, tv.sd >= 0 ? shape[tv.sd] : 1, false,
+                [&](int dev, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(dev);
+    if (rc) return rc;
+    ThetaPlan tp = plan;
+    rc = upload_theta(ss, &tp, theta, theta_strides);
+    if (rc) return rc;
+    const void* d_bins = nullptr;
+    rc = ss.upload(kAuxTarget, target_bins, (size_t)m * es, &d_bins);
+    if (rc) return rc;
+    rc = ss.fence();
+    if (rc) return rc;
+    rc = plan_theta_bounds(ss, &tp, theta_strides);
+    if (rc) return rc;
+    void* outs[1] = {out};
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM], th_strides[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
+      if (tv.sd >= 0) sshape[tv.sd] = j1 - j0;
+      const void* th = nullptr;
+      const int rc2 = tp.slab(j0, j1, b, st, &th, th_strides);
+      if (rc2) return rc2;
+      return xg_vinterp_conservative(dtype, b.in, th, th_strides, d_bins, m, flip_out, b.out[0], ndim, sshape, axis,
+                                     st);
+    };
+    return ss.run(es, phi, tv.vin, 1, outs, &tv.vout, launch, tv.ex.rows(r0, r1));
+  });
 }

@@ -7,7 +7,7 @@ compute path: without a CUDA device these helpers raise.
 
 from __future__ import annotations
 
-from typing import Tuple
+from typing import Sequence, Tuple
 
 import numpy as np
 import torch
@@ -71,6 +71,38 @@ def as_device_constant(data, device=None) -> torch.Tensor:
         hit = torch.from_numpy(arr.copy()).to(dev)
         _small_cache[key] = hit
     return hit
+
+
+_host_groups: dict = {}
+
+
+def host_group(devices: Sequence[int]) -> int:
+    """Handle of the host device group ``devices`` (``xg_host_group``), cached per member list.
+
+    Passed as the ``device`` of an ``ops.*_host`` call, it spreads the call's slabs over the members: the result
+    rows are cut into one contiguous block per member, and each member streams its block through its own PCIe
+    link.  A member may repeat; its blocks then take turns on that GPU."""
+    key = tuple(int(d) for d in devices)
+    hit = _host_groups.get(key)
+    if hit is None:
+        import ctypes as C
+
+        from . import _capi
+
+        handle = C.c_int(0)
+        _capi.check(_capi.load().xg_host_group(len(key), (C.c_int * max(len(key), 1))(*key), C.byref(handle)))
+        hit = _host_groups[key] = handle.value
+    return hit
+
+
+def host_device_arg(device) -> int:
+    """The ``int device`` argument of a ``*_host`` entry point: the current CUDA device for None, an index, or the
+    handle of the group a sequence of indices names."""
+    if device is None:
+        return torch.cuda.current_device()
+    if isinstance(device, (int, np.integer)):
+        return int(device)
+    return host_group(device)
 
 
 def result_like(t: torch.Tensor, was_host: bool):

@@ -53,8 +53,27 @@ def _maybe_promote_str_to_list(a):
     return [a] if isinstance(a, str) else a
 
 
+def _host_devices_arg(host_devices):
+    """``Grid(host_devices=...)``: None, "all", or a non-empty tuple of CUDA device indices."""
+    if host_devices is None or (isinstance(host_devices, str) and host_devices == "all"):
+        return host_devices
+    if isinstance(host_devices, (str, bytes)) or not isinstance(host_devices, Iterable):
+        raise TypeError(f"host_devices must be None, 'all' or a sequence of CUDA device indices, got {host_devices!r}")
+    devices = tuple(host_devices)
+    if not devices or not all(isinstance(d, (int, np.integer)) and not isinstance(d, bool) and d >= 0
+                              for d in devices):
+        raise ValueError(f"host_devices must hold one or more non-negative CUDA device indices, got {host_devices!r}")
+    return tuple(int(d) for d in devices)
+
+
 class Grid:
-    """A collection of :class:`Axis` objects plus grid metrics, bound to a dataset."""
+    """A collection of :class:`Axis` objects plus grid metrics, bound to a dataset.
+
+    ``device``: the CUDA device of the calls on numpy fields (default: the current one).  ``host_devices``: None,
+    a sequence of CUDA device indices, or "all" (every visible GPU): calls that stream numpy fields through the GPU
+    in slabs spread those slabs over these GPUs, each streaming a contiguous block of the result through its own
+    PCIe link.  Results are bit for bit those of one GPU.  Device tensors, and numpy fields on routes that do not
+    stream, keep using ``device``."""
 
     def __init__(
         self,
@@ -67,6 +86,7 @@ class Grid:
         metrics: Optional[Mapping[Tuple[str], List[str]]] = None,
         autoparse_metadata: bool = True,
         device=None,
+        host_devices=None,
         **kwargs,
     ):
         if "boundary" in kwargs:
@@ -85,6 +105,7 @@ class Grid:
             self._xarray_io = True
         self._ds = ds
         self._device = device
+        self._host_devices = _host_devices_arg(host_devices)
 
         if autoparse_metadata and coords is None:
             from .metadata import parse_comodo
@@ -272,6 +293,17 @@ class Grid:
         from .device import default_device
 
         return default_device()
+
+    def _host_device(self, da=None):
+        """The ``device`` of the ``ops.*_host`` call that streams numpy field ``da``: the grid's ``host_devices``
+        group when it has one, else the index of the CUDA device the call runs on."""
+        if self._host_devices is None:
+            return self._device_for(da).index
+        if self._host_devices == "all":
+            import torch
+
+            return tuple(range(torch.cuda.device_count()))
+        return self._host_devices
 
     def _metric_tensor(self, metric: DataArray, field_dims: Sequence[str], like):
         """Device tensor of ``metric`` shaped to broadcast against ``field_dims`` (size-1 elsewhere)."""
@@ -611,7 +643,7 @@ class Grid:
             # numpy-backed field: slabs stream through the GPU (xg_stencil_multi_host), so input, result and the
             # device footprint need not fit in HBM together
             try:
-                out = ops.stencil_multi_host(np.asarray(array.data), specs, device=dev.index)
+                out = ops.stencil_multi_host(np.asarray(array.data), specs, device=self._host_device(array))
             except NotImplementedError:
                 out = None  # a cut along an operated dim the slabs cannot pad: the whole field on the device
         if out is None:
@@ -689,8 +721,7 @@ class Grid:
             fv = fills[ax_name] if fills[ax_name] is not None else 0.0
             specs.append((axn, funcname, lo, hi, pad_mode if (lo or hi) else None, fv))
             renames.append((in_dim, out_dim, ax_name, (lo, hi)))
-        dev = self._device_for(da)
-        outs = ops.stencil2_host_multi(np.asarray(da.data), specs, device=dev.index)
+        outs = ops.stencil2_host_multi(np.asarray(da.data), specs, device=self._host_device(da))
         results = []
         for arr, (in_dim, out_dim, ax_name, width) in zip(outs, renames):
             out_dims = tuple(out_dim if d == in_dim else d for d in da.dims)
@@ -827,7 +858,7 @@ class Grid:
                 def cut(a):
                     return None if a is None else _merge_leading(a, ndrop, nmerge)
 
-                kw = dict(pre_a=cut(pre_a), pre_b=cut(pre_b), post=cut(post), device=dev.index)
+                kw = dict(pre_a=cut(pre_a), pre_b=cut(pre_b), post=cut(post), device=self._host_device(da_a))
                 spec_b = (spec_b[0] - shift,) + spec_b[1:]
                 if second["folded"]:
                     _, seam, skip, mirror, period = _fold_plan(self, second["ax"], dims, shape, 1)
@@ -1021,7 +1052,7 @@ class Grid:
                 y = ops.cumscan_host(
                     np.asarray(data.data), axis_num, ax_reverse, trim, pad_lo, pad_hi,
                     ax_padding if (pad_lo or pad_hi) else None, fv, pre=pre_t, post=post_t, skipna=True,
-                    device=self._device_for(da).index,
+                    device=self._host_device(da),
                 )
             else:
                 y = ops.cumscan(
@@ -1069,7 +1100,7 @@ class Grid:
             arr = np.asarray(da.data)
             axn = da.get_axis_num(dims[0])
             w_np = self._metric_host(weight, da.dims, arr.dtype)
-            y = ops.wreduce_host(arr, axn, w_np, mode, bool(skipna), device=self._device_for(da).index)
+            y = ops.wreduce_host(arr, axn, w_np, mode, bool(skipna), device=self._host_device(da))
             res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ != dims[0]), name=da.name)
             coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
             return self._wrap_out(res.assign_coords(coords), as_xarray)
@@ -1082,7 +1113,7 @@ class Grid:
             w_np = self._metric_host(weight, da.dims, arr.dtype)
             try:
                 y = ops.wreduce_host_multi(arr, [da.get_axis_num(d) for d in dims], w_np, mode, bool(skipna),
-                                           device=dev.index)
+                                           device=self._host_device(da))
             except NotImplementedError:
                 y = None  # an empty reduced dim, or a single line: the whole field on the device
             if y is not None:

@@ -644,7 +644,7 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             x = cut(da.data)
             ax = axis_num - ndrop - nmerge + 1
             kw = dict(pre=None if pre_h is None else cut(pre_h), post=None if post_h is None else cut(post_h),
-                      device=grid._device_for(da).index)
+                      device=grid._host_device(da))
             try:
                 if folded:
                     _, seam, skip, mirror, period = _fold_plan(grid, ax_name, dims, shape, 1)
@@ -754,7 +754,7 @@ def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_di
                                      partner_layout)
     out = ops.stencil2_host_connected(x, m_dims.index(in_dim), op, lo, hi, fv, program, partner=q,
                                       post=None if post_h is None else cut(post_h),
-                                      device=grid._device_for(da).index)
+                                      device=grid._host_device(da))
     return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
 
 

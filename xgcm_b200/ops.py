@@ -7,12 +7,17 @@ There is no CPU path: a non-CUDA tensor raises.
 
 from __future__ import annotations
 
-from typing import Optional, Sequence, Tuple
+from typing import Optional, Sequence, Tuple, Union
 
 import numpy as np
 import torch
 
 from . import _capi
+from .device import host_device_arg
+
+# the `device` of the *_host functions: None (the current CUDA device), an index, or a sequence of indices, a host
+# device group that spreads the call's slabs over those GPUs (device.host_group)
+HostDevice = Optional[Union[int, Sequence[int]]]
 
 _TORCH_DTYPE_CODE = {torch.float32: _capi.XG_F32, torch.float64: _capi.XG_F64}
 
@@ -569,7 +574,7 @@ def stencil2_host(
     pre: Optional[np.ndarray] = None,
     post: Optional[np.ndarray] = None,
     out: Optional[np.ndarray] = None,
-    device: Optional[int] = None,
+    device: HostDevice = None,
 ) -> np.ndarray:
     """Host-buffer twin of :func:`stencil2`: slabs stream H2D -> kernel -> D2H on three
     streams inside ``xg_stencil2_host``.  Page-locked buffers get the full PCIe rate."""
@@ -610,14 +615,14 @@ def _host_stencil_prep(x, axis, op, lo, hi, padding, pre, post, out, device, wha
         raise ValueError("out has wrong shape/dtype/layout")
     pre_op = _host_operand(pre, shape, x.dtype, "pre metric")
     post_op = _host_operand(post, out_shape, x.dtype, "post metric")
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     return x, shape, axis, out, pre_op, post_op, dev
 
 
 def stencil2_host_fold(x: np.ndarray, axis: int, op: str, lo: int, hi: int, padding: Optional[str],
                        fill_value: float, seam_axis: int, skip: int, mirror: int, period: int,
                        negate: bool = False, pre: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None,
-                       out: Optional[np.ndarray] = None, device: Optional[int] = None) -> np.ndarray:
+                       out: Optional[np.ndarray] = None, device: HostDevice = None) -> np.ndarray:
     """:func:`stencil2_host` across a north fold along ``axis`` (``xg_stencil2_host_fold``): each slab's
     halo_hi is its folded row (:func:`fold_rows` with ``seam_axis, skip, mirror, period, negate``, of
     ``x * pre``), also halo_lo when the south edge ``padding`` is periodic.  Dim 0 is cut into slabs and must
@@ -641,7 +646,7 @@ _HALO_SOURCES = {"self": 0, "partner": 1, "fill": 2}
 def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int, fill_value: float,
                             program: Sequence[tuple], partner: Optional[np.ndarray] = None,
                             post: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
-                            device: Optional[int] = None) -> np.ndarray:
+                            device: HostDevice = None) -> np.ndarray:
     """:func:`stencil2_host` on a grid with face connections (``xg_stencil2_host_connected``): the halo
     planes of each slab are written by ``program``, the strided copies of
     ``padding.connected_halo_program`` — ``(side, dst offset, dst strides, source ("self", "partner" or
@@ -752,14 +757,14 @@ def _host_pair_prep(a, b, spec_a, spec_b, pre_a, pre_b, post, out, device, what)
         raise ValueError("out has wrong shape/dtype/layout")
     ops_ = [_host_operand(m, shape, a.dtype, w) for m, w in ((pre_a, "pre metric a"), (pre_b, "pre metric b"),
                                                              (post, "post metric"))]
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     return a, b, shape, term_a, term_b, ops_, out, dev
 
 
 def stencil_pair_host(a: np.ndarray, b: np.ndarray, spec_a, spec_b, subtract: int = 0,
                       pre_a: Optional[np.ndarray] = None, pre_b: Optional[np.ndarray] = None,
                       post: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
-                      device: Optional[int] = None) -> np.ndarray:
+                      device: HostDevice = None) -> np.ndarray:
     """Host-buffer twin of :func:`stencil_pair` (``xg_stencil_pair_host``): ``a`` and ``b`` stream through the
     GPU in slabs of dim 0, which must be a batch dim (not ``spec_b``'s axis)."""
     lib = _capi.load()
@@ -775,7 +780,7 @@ def stencil_pair_host(a: np.ndarray, b: np.ndarray, spec_a, spec_b, subtract: in
 def stencil_pair_host_fold(a: np.ndarray, b: np.ndarray, spec_a, spec_b, seam_axis: int, skip: int, mirror: int,
                            period: int, subtract: int = 0, negate: bool = False, pre_a: Optional[np.ndarray] = None,
                            pre_b: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None,
-                           out: Optional[np.ndarray] = None, device: Optional[int] = None) -> np.ndarray:
+                           out: Optional[np.ndarray] = None, device: HostDevice = None) -> np.ndarray:
     """:func:`stencil_pair_host` with the term along ``spec_b``'s axis across a north fold
     (``xg_stencil_pair_host_fold``): each slab's ``halo_hi_b`` is the folded row of ``b * pre_b``
     (:func:`fold_rows` with ``seam_axis, skip, mirror, period, negate``), also ``halo_lo_b`` when ``spec_b``
@@ -804,7 +809,7 @@ def _host_field(x, what):
     return x
 
 
-def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: Optional[int] = None):
+def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: HostDevice = None):
     """One host field up, several stencil results down (``xg_stencil2_host_multi``).
 
     ``specs``: sequence of ``(axis, op, lo, hi, padding, fill_value)``.  Returns a list of page-locked
@@ -838,7 +843,7 @@ def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: Optional[int] =
     import ctypes as C
 
     out_ptrs = (C.c_void_p * k)(*[o.ctypes.data for o in outs])
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     rc = lib.xg_stencil2_host_multi(
         k, (C.c_int * k)(*ops_), _capi.dtype_code(x.dtype), x.ctypes.data, out_ptrs, x.ndim,
         _capi.i64_array(shape), (C.c_int * k)(*axes), (C.c_int * k)(*los), (C.c_int * k)(*his),
@@ -848,7 +853,7 @@ def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: Optional[int] =
 
 
 def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, Optional[str], float]],
-                       device: Optional[int] = None) -> np.ndarray:
+                       device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`stencil_multi` (``xg_stencil_multi_host``): slabs of the outermost non-operated dim of
     extent > 1 stream through the GPU, one fused launch each.  Raises NotImplementedError for what the slabs do not
     cover (mixed operators; an outer / inner shift or a periodic boundary along the cut dim when every dim of extent
@@ -882,7 +887,7 @@ def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, 
     out = pinned_empty(out_shape, x.dtype)
     n = len(specs)
     IntArr, DblArr = C.c_int * n, C.c_double * n
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size:
         rc = lib.xg_stencil_multi_host(
             _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), n,
@@ -894,7 +899,7 @@ def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, 
 def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "none", pad_lo: int = 0,
                  pad_hi: int = 0, padding: Optional[str] = None, fill_value: float = 0.0,
                  pre: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None, skipna: bool = True,
-                 device: Optional[int] = None) -> np.ndarray:
+                 device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`cumscan` (``xg_cumscan_host``): slabs of a non-operated dim stream through the GPU."""
     lib = _capi.load()
     x = _host_field(x, "field")
@@ -910,7 +915,7 @@ def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "n
     out = pinned_empty(out_shape, x.dtype)
     kp, pre_ptr, pre_st = _host_operand(pre, shape, x.dtype, "pre metric")
     kq, post_ptr, post_st = _host_operand(post, out_shape, x.dtype, "post metric")
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size:
         rc = lib.xg_cumscan_host(
             _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), axis,
@@ -921,7 +926,7 @@ def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "n
 
 
 def wreduce_host(x: np.ndarray, axis: int, weight: Optional[np.ndarray] = None, mode: str = "sum",
-                 skipna: bool = True, device: Optional[int] = None) -> np.ndarray:
+                 skipna: bool = True, device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`wreduce` (``xg_wreduce_host``)."""
     lib = _capi.load()
     x = _host_field(x, "field")
@@ -930,7 +935,7 @@ def wreduce_host(x: np.ndarray, axis: int, weight: Optional[np.ndarray] = None, 
     out_shape = [s for d, s in enumerate(shape) if d != axis]
     out = pinned_empty(out_shape if out_shape else [1], x.dtype)
     kw, w_ptr, w_st = _host_operand(weight, shape, x.dtype, "weight")
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size and x.size:
         rc = lib.xg_wreduce_host(_capi.dtype_code(x.dtype), x.ctypes.data, w_ptr, w_st, out.ctypes.data, x.ndim,
                                  _capi.i64_array(shape), axis, _capi.REDUCE[mode], int(bool(skipna)), dev)
@@ -939,7 +944,7 @@ def wreduce_host(x: np.ndarray, axis: int, weight: Optional[np.ndarray] = None, 
 
 
 def wreduce_host_multi(x: np.ndarray, axes: Sequence[int], weight: Optional[np.ndarray] = None, mode: str = "sum",
-                       skipna: bool = True, device: Optional[int] = None) -> np.ndarray:
+                       skipna: bool = True, device: HostDevice = None) -> np.ndarray:
     """Weighted sum / mean of a host field over several ``axes`` (``xg_wreduce_host_multi``), bit for bit the
     chain of :func:`wreduce` calls ``Grid.integrate`` / ``Grid.average`` run on the device.  Raises
     NotImplementedError for what the slabs do not cover (an empty reduced dim, or no reduced dim of extent > 1
@@ -953,7 +958,7 @@ def wreduce_host_multi(x: np.ndarray, axes: Sequence[int], weight: Optional[np.n
     out_shape = [s for d, s in enumerate(shape) if d not in axes]
     out = pinned_empty(out_shape if out_shape else [1], x.dtype)
     kw, w_ptr, w_st = _host_operand(weight, shape, x.dtype, "weight")
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size:
         n = len(axes)
         rc = lib.xg_wreduce_host_multi(_capi.dtype_code(x.dtype), x.ctypes.data, w_ptr, w_st, out.ctypes.data,
@@ -965,7 +970,7 @@ def wreduce_host_multi(x: np.ndarray, axes: Sequence[int], weight: Optional[np.n
 
 def vinterp_linear_host(phi: np.ndarray, theta: np.ndarray, target: np.ndarray, axis: int,
                         mask_edges: bool = False, bypass_checks: bool = False, logarithmic: bool = False,
-                        device: Optional[int] = None) -> np.ndarray:
+                        device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`vinterp_linear` for a shared 1-D ``target`` (``xg_vinterp_linear_host``); ``theta``
     broadcasts against ``phi`` (the 1-D coordinate or a full field)."""
     lib = _capi.load()
@@ -984,7 +989,7 @@ def vinterp_linear_host(phi: np.ndarray, theta: np.ndarray, target: np.ndarray, 
     kt, th_ptr, th_st = _host_operand(theta, shape, phi.dtype, "theta")
     out_shape = [s for d, s in enumerate(shape) if d != axis] + [m]
     out = pinned_empty(out_shape, phi.dtype)
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size:
         rc = lib.xg_vinterp_linear_host(
             _capi.dtype_code(phi.dtype), phi.ctypes.data, th_ptr, th_st, target.ctypes.data, None, m,
@@ -995,7 +1000,7 @@ def vinterp_linear_host(phi: np.ndarray, theta: np.ndarray, target: np.ndarray, 
 
 
 def vinterp_conservative_host(phi: np.ndarray, theta: np.ndarray, target_bins: np.ndarray, axis: int,
-                              theta_at_centers: bool = False, device: Optional[int] = None) -> np.ndarray:
+                              theta_at_centers: bool = False, device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`vinterp_conservative` (``xg_vinterp_conservative_host``): slabs of ``phi`` (and of
     ``theta`` when it is a full field) stream through the GPU.  With ``theta_at_centers``, ``theta`` holds n
     cell-centre values along ``axis`` and its bounds are those of ``grid.interp(theta, axis, padding="extend")``."""
@@ -1027,7 +1032,7 @@ def vinterp_conservative_host(phi: np.ndarray, theta: np.ndarray, target_bins: n
     m = int(bins.size)
     out_shape = [s for d, s in enumerate(shape) if d != axis] + [m - 1]
     out = pinned_empty(out_shape, phi.dtype)
-    dev = torch.cuda.current_device() if device is None else int(device)
+    dev = host_device_arg(device)
     if out.size:
         rc = lib.xg_vinterp_conservative_host(
             _capi.dtype_code(phi.dtype), phi.ctypes.data, th_ptr, th_st, int(bool(theta_at_centers)),

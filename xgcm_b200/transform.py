@@ -76,7 +76,7 @@ def linear_interpolation(phi, theta, target_theta_levels, phi_dim, theta_dim, ta
         th = th.reshape([sizes[d] if d in th_dims else 1 for d in phi.dims])
         out = ops.vinterp_linear_host(np.asarray(phi.data), th, np.asarray(target_theta_levels.values),
                                       phi.get_axis_num(phi_dim), mask_edges, bypass_checks, logarithmic,
-                                      device=None if device is None else device.index)
+                                      device=None if grid is None else grid._host_device(phi))
         out_dims = tuple(d for d in phi.dims if d != phi_dim) + (target_dim,)
         coords = {k: c for k, c in phi.coords.items()
                   if phi_dim not in c.dims and k != target_dim and all(d in out_dims for d in c.dims)}
@@ -227,7 +227,8 @@ def _conservative_interpolation(phi, theta, target_theta_levels, phi_dim, theta_
             raise ValueError(f"`target_data` needs {need} {what} along {theta_dim!r}, got {sizes[phi_dim]}")
         th = th.reshape([sizes[d] if d in th_dims else 1 for d in phi.dims])
         out = ops.vinterp_conservative_host(np.asarray(phi.data), th, np.asarray(target_theta_levels.values),
-                                            phi.get_axis_num(phi_dim), theta_at_centers, device=host_dev.index)
+                                            phi.get_axis_num(phi_dim), theta_at_centers,
+                                            device=host_dev.index if grid is None else grid._host_device(phi))
         return _conservative_result(out, phi, phi_dim, target_theta_levels, target_dim, suffix)
     device = grid._device_for(phi) if grid is not None else None
     x, host = as_device_tensor(phi.data, device)
