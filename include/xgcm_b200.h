@@ -437,6 +437,37 @@ XG_API int xg_cumscan_host(int dtype, const void* in, void* out, int ndim, const
 XG_API int xg_wreduce_host(int dtype, const void* in, const void* weight, const int64_t* w_strides,
                     void* out, int ndim, const int64_t* shape, int axis, int mode, int skipna,
                     int device);
+
+/*
+ * xg_cumscan_host on the two grid topologies whose halo is not a boundary condition: Grid.cumsum / cumint of a
+ * HOST field whose padded edge takes its halo across a north fold or a face connection.  Same result, bit for bit,
+ * as the device sequence scan -> pad() -> divide: per slab, xg_cumscan (pre_metric, reverse, trim; no pad, no
+ * post) into workspace scratch; the halo planes taken from the SCANNED slab (the field's shape with `trim` applied,
+ * extent 1 along `axis`); one xg_strided_copy_batch launch writing the scanned slab and its planes into the padded
+ * result; one xg_binary launch dividing it by `post_metric` (broadcast against the result's shape).  The slab
+ * pipeline of xg_stencil2_host_fold / _connected: dim 0 is cut into slabs and must be a batch dim, not the scanned,
+ * seam or face dim (XG_EINVAL); device memory is bounded by the slab size plus the whole-call metrics.  Every
+ * argument is checked before any CUDA call.
+ *
+ * _fold: the north halo of a reverse scan (pad_lo = 0, pad_hi = 1, no other edge to pad: no bc) is one
+ * xg_fold_rows launch on the scanned slab (width 1; seam_axis, skip, mirror, period as there, for the scanned
+ * shape).  XG_ENOTIMPL where xg_fold_rows would return it.
+ *
+ * _connected: the halo planes are written by the copy list of xg_stencil2_host_connected (no partner: source 0 is
+ * the scanned field, 2 the constant fill_value), described for the whole SCANNED field; it covers the unconnected
+ * edges with their basic boundary too, so there is no bc.
+ */
+XG_API int xg_cumscan_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,
+                                int reverse, int trim, int pad_lo, int pad_hi, const void* pre_metric,
+                                const int64_t* pre_strides, const void* post_metric, const int64_t* post_strides,
+                                int skipna, int seam_axis, int skip, int64_t mirror, int64_t period, int device);
+XG_API int xg_cumscan_host_connected(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                     int axis, int reverse, int trim, int pad_lo, int pad_hi, double fill_value,
+                                     const void* pre_metric, const int64_t* pre_strides, const void* post_metric,
+                                     const int64_t* post_strides, int skipna, int ncopies, int copy_ndim,
+                                     const int* side, const int* source, const int64_t* dst_offset,
+                                     const int64_t* src_offset, const int64_t* shapes, const int64_t* dst_strides,
+                                     const int64_t* src_strides, const int* negate, int device);
 XG_API int xg_vinterp_linear_host(int dtype, const void* phi, const void* theta,
                            const int64_t* theta_strides, const void* target,
                            const int64_t* target_strides, int64_t m, void* out, int ndim,

@@ -1,14 +1,17 @@
 """Numpy fields on face-connected and north-fold grids through the host slab pipelines, beside the plain-grid
 host call on the same shape (the ceiling: same slabs, no halo stage) and beside the old whole-field route
-(upload, device call, download).  Page-locked inputs, host clock around each synchronous call, the variants
-alternated `--rounds` times in one process.  Prints one JSON line with the card, its power limit, the median
-seconds and GB/s (bytes in + out over time) of every variant, and tools/bench_pcie.py's copy rates.
+(upload, device call, download): Grid.diff, and Grid.cumsum across the faces (X to outer: a trimmed shift such as
+X to left raises across the cubed sphere's axis-swapping seams), along Z, and reversed across the fold.
+Page-locked inputs, host clock around each synchronous call, the variants alternated `--rounds` times in one
+process.  Prints one JSON line with the card, its power limit, the median seconds and GB/s (bytes in + out over
+time) of every variant, its ratio to the plain-grid ceiling and to the old route, and tools/bench_pcie.py's copy
+rates.
 
     python tools/bench_host_halo.py [--faces 90 6 2160 2160] [--fold 75 3059 4322] [--rounds 5]
 
 If MemAvailable allows about 2.2x of it, a year of monthly ORCA12-like temperature (12, 75, 3059, 4322) fp32
-(47.6 GB) also streams across the fold, with sampled time steps checked against oracle/fold.py.  The old
-route runs only where input, partner and output fit on the card with room to spare.
+(47.6 GB) also streams across the fold (diff, then the reverse cumsum), with sampled time steps checked against
+oracle/fold.py.  The old route runs only where its device buffers fit on the card with room to spare.
 """
 
 import argparse
@@ -83,13 +86,14 @@ def old_route(grid, method, da, dims, other=None, **kw):
 
 def faces_variants(shape):
     nt, nf, ny, nx = shape
-    coords = {"x": np.arange(nx) + 0.0, "xl": np.arange(nx) - 0.5, "y": np.arange(ny) + 0.0,
-              "yl": np.arange(ny) - 0.5, "face": np.arange(nf)}
+    coords = {"x": np.arange(nx) + 0.0, "xl": np.arange(nx) - 0.5, "xo": np.arange(nx + 1) - 0.5,
+              "y": np.arange(ny) + 0.0, "yl": np.arange(ny) - 0.5, "face": np.arange(nf), "k": np.arange(nt) + 0.0,
+              "kl": np.arange(nt) - 0.5}
     ds = xg.Dataset(coords=coords)
-    grid = xg.Grid(ds, coords={"X": {"center": "x", "left": "xl"}, "Y": {"center": "y", "left": "yl"}},
-                   face_connections=CUBED_SPHERE)
-    plain = xg.Grid(ds, coords={"X": {"center": "x", "left": "xl"}, "Y": {"center": "y", "left": "yl"}},
-                    padding="fill")
+    axes = {"X": {"center": "x", "left": "xl", "outer": "xo"}, "Y": {"center": "y", "left": "yl"},
+            "Z": {"center": "k", "left": "kl"}}
+    grid = xg.Grid(ds, coords=axes, face_connections=CUBED_SPHERE)
+    plain = xg.Grid(ds, coords=axes, padding="fill")
     c = pinned_random(shape, 1)
     v = pinned_random(shape, 2)
     cd, ud, vd = ("k", "face", "y", "x"), ("k", "face", "y", "xl"), ("k", "face", "yl", "x")
@@ -99,10 +103,17 @@ def faces_variants(shape):
         "faces_vector_diffX": lambda: grid.diff({"X": xg.DataArray(c, dims=ud)}, "X",
                                                 other_component={"Y": xg.DataArray(v, dims=vd)}, padding="fill"),
         "plain_diffX": lambda: plain.diff(xg.DataArray(c, dims=cd), "X"),
+        "faces_cumsumX": lambda: grid.cumsum(xg.DataArray(c, dims=cd), "X", to="outer"),
+        "plain_cumsumX": lambda: plain.cumsum(xg.DataArray(c, dims=cd), "X", to="outer"),
+        "faces_cumsumZ": lambda: grid.cumsum(xg.DataArray(c, dims=cd), "Z", padding="fill"),
+        "plain_cumsumZ": lambda: plain.cumsum(xg.DataArray(c, dims=cd), "Z"),
     }
     if fits:
         variants["faces_scalar_diffX_old"] = old_route(grid, "diff", c, cd, axis="X", padding="fill")
         variants["faces_vector_diffX_old"] = old_route(grid, "diff", c, ud, {"Y": (v, vd)}, axis="X", padding="fill")
+    if 4 * c.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:  # input, scan, padded copy, result
+        variants["faces_cumsumX_old"] = old_route(grid, "cumsum", c, cd, axis="X", to="outer")
+        variants["faces_cumsumZ_old"] = old_route(grid, "cumsum", c, cd, axis="Z", padding="fill")
     return variants, 2 * c.nbytes, {"faces_vector_diffX": 3 * c.nbytes, "faces_vector_diffX_old": 3 * c.nbytes}
 
 
@@ -124,9 +135,14 @@ def fold_variants(shape):
     variants = {
         "fold_diffY": lambda: grid.diff(xg.DataArray(a, dims=dims), "Y", to="center"),
         "plain_fold_shape_diffY": lambda: plain.diff(xg.DataArray(a, dims=dims), "Y", to="center"),
+        "fold_cumsumY_reverse": lambda: grid.cumsum(xg.DataArray(a, dims=dims), "Y", to="center", reverse=True),
+        "plain_fold_shape_cumsumY_reverse": lambda: plain.cumsum(xg.DataArray(a, dims=dims), "Y", to="center",
+                                                                 reverse=True),
     }
     if 2 * a.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:
         variants["fold_diffY_old"] = old_route(grid, "diff", a, dims, axis="Y", to="center")
+    if 4 * a.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:  # input, scan, padded copy, result
+        variants["fold_cumsumY_reverse_old"] = old_route(grid, "cumsum", a, dims, axis="Y", to="center", reverse=True)
     return variants, 2 * a.nbytes, {}
 
 
@@ -150,17 +166,26 @@ def orca_year(rounds):
     grid, _ = fold_grid(shape[2], shape[3])
     a = pinned_random(shape, 4)
     da = xg.DataArray(a, dims=("t", "z", "yl", "xc"))
-    ts = []
-    for _ in range(max(1, rounds // 2)):
-        out = [None]
-        ts.append(timed_call(lambda: out.__setitem__(0, grid.diff(da, "Y", to="center"))))
-    got = out[0].data
     roles = F.resolve_pivot("T", "Y", "X")
-    for t, z in ((0, 0), (5, 40), (11, 74)):
-        padded = F.pad_fold(a[t, z], 0, 1, "left", "center", roles, {0: (0, 1)}, {0: "fill"})
-        np.testing.assert_array_equal(got[t, z], S.stencil2("diff", padded, 0, 0, 0, None))
-    return {"shape": shape, "s": statistics.median(ts), "GBps": 2 * nbytes / statistics.median(ts) / 1e9,
-            "checked_steps": [[0, 0], [5, 40], [11, 74]]}
+    steps = ((0, 0), (5, 40), (11, 74))
+    result = {"shape": shape, "checked_steps": [list(s) for s in steps]}
+    for name, call, want in (
+            ("diffY", lambda: grid.diff(da, "Y", to="center"),
+             lambda s: S.stencil2("diff", F.pad_fold(s, 0, 1, "left", "center", roles, {0: (0, 1)}, {0: "fill"}),
+                                  0, 0, 0, None)),
+            ("cumsumY_reverse", lambda: grid.cumsum(da, "Y", to="center", reverse=True),
+             lambda s: F.pad_fold(S.cumscan(s, 0, True, "drop_first"), 0, 1, "left", "center", roles, {0: (0, 1)},
+                                  {0: "fill"}))):
+        ts = []
+        for _ in range(max(1, rounds // 2)):
+            out = [None]
+            ts.append(timed_call(lambda: out.__setitem__(0, call())))
+        got = out[0].data
+        for t, z in steps:
+            np.testing.assert_array_equal(got[t, z], want(a[t, z]))
+        del out, got
+        result[name] = {"s": statistics.median(ts), "GBps": 2 * nbytes / statistics.median(ts) / 1e9}
+    return result
 
 
 def main():
@@ -189,9 +214,13 @@ def main():
             result[k] = {"s": med, "min_s": min(ts), "GBps": moved_by.get(k, moved) / med / 1e9}
         del variants
     for name, ceiling in (("faces_scalar_diffX", "plain_diffX"), ("faces_vector_diffX", "plain_diffX"),
-                          ("fold_diffY", "plain_fold_shape_diffY")):
+                          ("fold_diffY", "plain_fold_shape_diffY"), ("faces_cumsumX", "plain_cumsumX"),
+                          ("faces_cumsumZ", "plain_cumsumZ"),
+                          ("fold_cumsumY_reverse", "plain_fold_shape_cumsumY_reverse")):
         if name in result and ceiling in result:
             result[name]["vs_plain"] = result[name]["s"] / result[ceiling]["s"]
+        if name in result and name + "_old" in result:
+            result[name]["vs_old"] = result[name]["s"] / result[name + "_old"]["s"]
     result["orca_year"] = {"skipped": "--skip-year"} if args.skip_year else orca_year(args.rounds)
     print(json.dumps(result))
 

@@ -110,6 +110,16 @@ SIGNATURES = {
         [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
          C.c_double, _vp, _i64p, _vp, _i64p, C.c_int, C.c_int],
     ),
+    "xg_cumscan_host_fold": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _i64p, _vp, _i64p,
+         C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int],
+    ),
+    "xg_cumscan_host_connected": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p,
+         _vp, _i64p, C.c_int, C.c_int, C.c_int, _i32p, _i32p, _i64p, _i64p, _i64p, _i64p, _i64p, _i32p, C.c_int],
+    ),
     "xg_wreduce_host": (
         C.c_int,
         [C.c_int, _vp, _vp, _i64p, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int],

@@ -24,7 +24,9 @@
 // face-connection copy list clipped to the slab and replayed with xg_strided_copy_batch) just before its
 // xg_stencil2 launch.  xg_stencil_pair_host / xg_stencil_pair_host_fold: field a is the slab input, field b the
 // second streamed input, and each slab is one xg_stencil_pair_halo launch (after the xg_fold_rows launch of b's
-// folded row, for the fold).
+// folded row, for the fold).  xg_cumscan_host_fold / xg_cumscan_host_connected run the same halo stages on each
+// slab's scanned rows (xg_cumscan into the scratch buffer), then place the scanned slab and its halo planes into the
+// padded result slab and divide by the post-metric.
 #include <stdlib.h>
 
 #include <thread>
@@ -573,6 +575,228 @@ void copy_extent(int64_t offset, const int64_t* strides, const int64_t* shape, i
   }
 }
 
+// The face-connection copy list of the _connected entry points, described once for the whole field (see the header).
+struct CopyList {
+  int n, ndim;
+  const int *side, *source;
+  const int64_t *dst_offset, *src_offset, *shapes, *dst_strides, *src_strides;
+  const int* negate;
+};
+
+// The copy-list checks, before any CUDA call: each copy writes a padded halo plane (plane_row elements per dim-0
+// index of n0) from the field (row_in per index), the partner (partner_row, when given) or the fill constant, spans
+// dim 0 in full, and stays inside both arrays; together the copies cover each padded plane.  *fill: some copy reads
+// the constant.
+int validate_copies(const std::string& who, const CopyList& cl, int lo, int hi, int64_t n0, int64_t plane_row,
+                    int64_t row_in, bool partner, int64_t partner_row, bool* fill) {
+  if (cl.n < 0) return xg_fail(XG_EINVAL, who + ": negative copy count");
+  if (cl.n > 0 && (!cl.side || !cl.source || !cl.dst_offset || !cl.src_offset || !cl.shapes || !cl.dst_strides ||
+                   !cl.src_strides || !cl.negate))
+    return xg_fail(XG_EINVAL, who + ": null pointer in the copy list");
+  if (cl.n > 0 && (cl.ndim < 1 || cl.ndim > XG_MAX_NDIM)) return xg_fail(XG_EINVAL, who + ": bad copy rank");
+  int64_t covered[2] = {0, 0};
+  *fill = false;
+  for (int k = 0; k < cl.n; ++k) {
+    const int64_t* sh = cl.shapes + (size_t)k * cl.ndim;
+    const int64_t* ds = cl.dst_strides + (size_t)k * cl.ndim;
+    const int64_t* ss = cl.src_strides + (size_t)k * cl.ndim;
+    const int side = cl.side[k], source = cl.source[k];
+    const std::string at = who + ": copy " + std::to_string(k) + ": ";
+    if (side != 0 && side != 1) return xg_fail(XG_EINVAL, at + "side must be 0 (lo) or 1 (hi)");
+    if (!(side ? hi : lo)) return xg_fail(XG_EINVAL, at + "writes a halo plane the call does not pad");
+    if (source < kSrcField || source > kSrcFill)
+      return xg_fail(XG_EINVAL, at + "source must be 0 (field), 1 (partner) or 2 (fill constant)");
+    if (source == kSrcPartner && !partner) return xg_fail(XG_EINVAL, at + "reads a partner that was not given");
+    *fill = *fill || source == kSrcFill;
+    int64_t cells = 1;
+    for (int d = 0; d < cl.ndim; ++d) {
+      if (sh[d] < 0) return xg_fail(XG_EINVAL, at + "negative extent");
+      cells *= sh[d];
+    }
+    covered[side] += cells;
+    const int64_t src_row = source == kSrcField ? row_in : source == kSrcPartner ? partner_row : 0;
+    if (sh[0] != n0 || ds[0] != plane_row || ss[0] != src_row)
+      return xg_fail(XG_EINVAL, at + "must span dim 0 in full with the contiguous dim-0 strides");
+    if (cells == 0) continue;
+    int64_t a, b;
+    copy_extent(cl.dst_offset[k], ds, sh, cl.ndim, &a, &b);
+    if (a < 0 || b >= n0 * plane_row) return xg_fail(XG_EINVAL, at + "leaves the halo plane");
+    copy_extent(cl.src_offset[k], ss, sh, cl.ndim, &a, &b);
+    if (source == kSrcFill) {
+      if (a != 0 || b != 0) return xg_fail(XG_EINVAL, at + "the fill constant is read with offset 0, strides 0");
+    } else if (a < 0 || b >= n0 * src_row) {
+      return xg_fail(XG_EINVAL, at + "leaves its source array");
+    }
+  }
+  // the copies write disjoint cells, so together they must cover each padded plane exactly once
+  if ((lo && covered[0] != n0 * plane_row) || (hi && covered[1] != n0 * plane_row))
+    return xg_fail(XG_EINVAL, who + ": the copies do not cover the halo planes");
+  return XG_OK;
+}
+
+// The face connections' halo stage: the whole-field copy list rebased onto the slab's buffers (the field is b.in, the
+// partner b.in2), `slab_shape[0]` rows high.  The rebased pointers and shapes are built per slab, on every path (three
+// vectors of cl.n entries, small beside a slab's copies): the stage then keeps no state between slabs, so the members
+// of a host device group can run it at once.
+HaloFn copy_stage(const CopyList& cl, int dtype, int lo, int hi) {
+  return [=](const SlabBufs& b, const int64_t* slab_shape, const void*, const void* d_fill, cudaStream_t st,
+             const void** hl, const void** hh) -> int {
+    const size_t es = dtype == XG_F32 ? 4 : 8;
+    std::vector<void*> dptr(cl.n);
+    std::vector<const void*> sptr(cl.n);
+    std::vector<int64_t> shp(cl.shapes ? cl.shapes : (const int64_t*)nullptr,
+                             cl.shapes ? cl.shapes + (size_t)cl.n * cl.ndim : (const int64_t*)nullptr);
+    for (int k = 0; k < cl.n; ++k) {
+      dptr[k] = static_cast<char*>(b.plane[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
+      const void* base = cl.source[k] == kSrcField ? b.in : cl.source[k] == kSrcPartner ? b.in2 : d_fill;
+      sptr[k] = static_cast<const char*>(base) + (size_t)cl.src_offset[k] * es;
+      shp[(size_t)k * cl.ndim] = slab_shape[0];
+    }
+    if (lo) *hl = b.plane[0];
+    if (hi) *hh = b.plane[1];
+    int rc2 = xg_strided_copy_batch(dtype, cl.n, dptr.data(), sptr.data(), cl.ndim, shp.data(), cl.dst_strides,
+                                    cl.src_strides, cl.negate, st);
+    if (rc2 != XG_ENOTIMPL) return rc2;
+    for (int k = 0; k < cl.n; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
+      rc2 = xg_strided_copy(dtype, dptr[k], cl.dst_strides + (size_t)k * cl.ndim, sptr[k],
+                            cl.src_strides + (size_t)k * cl.ndim, cl.ndim, shp.data() + (size_t)k * cl.ndim,
+                            cl.negate[k], st);
+      if (rc2) return rc2;
+    }
+    return XG_OK;
+  };
+}
+
+// ---------------------------------------------------------------------------------- the cumscan entry points
+// The arguments of xg_cumscan_host_fold / _connected.
+struct ScanCall {
+  int dtype;
+  const void* in;
+  void* out;
+  int ndim;
+  const int64_t* shape;
+  int axis, reverse, trim, pad_lo, pad_hi;
+  const void* pre;
+  const int64_t* pre_strides;
+  const void* post;
+  const int64_t* post_strides;
+  int skipna, device;
+};
+
+// The checks of xg_cumscan_host, plus those of the slab loop (dim 0 a batch dim), before any CUDA call.  *scan_shape:
+// the shape of the scanned field (trimmed, not yet padded), which the halo is taken from.
+int validate_scan_call(const char* who, const ScanCall& s, int64_t* scan_shape) {
+  const std::string w(who);
+  if (!s.in || !s.out || !s.shape) return xg_fail(XG_EINVAL, w + ": null pointer");
+  if (s.dtype != XG_F32 && s.dtype != XG_F64) return xg_fail(XG_EINVAL, w + ": dtype must be XG_F32 or XG_F64");
+  if (s.ndim < 1 || s.ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, w + ": bad ndim");
+  if (s.axis < 0 || s.axis >= s.ndim) return xg_fail(XG_EINVAL, w + ": axis out of range");
+  if (s.ndim < 2 || s.axis == 0)
+    return xg_fail(XG_EINVAL, w + ": dim 0 is cut into slabs and must not be the scanned dim");
+  for (int d = 0; d < s.ndim; ++d) {
+    if (s.shape[d] < 0) return xg_fail(XG_EINVAL, w + ": negative extent");
+    scan_shape[d] = s.shape[d];
+  }
+  if (s.trim < XG_TRIM_NONE || s.trim > XG_TRIM_DROP_FIRST) return xg_fail(XG_EINVAL, w + ": unknown trim");
+  if (s.pad_lo < 0 || s.pad_lo > 1 || s.pad_hi < 0 || s.pad_hi > 1)
+    return xg_fail(XG_EINVAL, w + ": pad widths must be 0 or 1");
+  if ((s.pre && !s.pre_strides) || (s.post && !s.post_strides))
+    return xg_fail(XG_EINVAL, w + ": metric strides missing");
+  scan_shape[s.axis] -= s.trim != XG_TRIM_NONE ? 1 : 0;
+  if (scan_shape[s.axis] < 1) return xg_fail(XG_EINVAL, w + ": no scanned row to take the halo from");
+  return XG_OK;
+}
+
+// A cumscan entry point with a halo (arguments checked) on s.device: the field in slabs along dim 0, the metrics
+// (and the `fill_host` constant, es bytes, when given) uploaded whole.  Per slab, the device sequence of
+// Grid.cumsum on such a grid: xg_cumscan (pre, reverse, trim; no pad, no post) into the scratch buffer; `halo` builds
+// the halo planes from the scanned slab; one xg_strided_copy_batch launch writes the scanned slab and its planes
+// into the padded result; one xg_binary launch divides it by `post` in place.
+int cumscan_halo_host(const char* who, const ScanCall& s, const int64_t* scan_shape, const HaloFn& halo,
+                      const void* fill_host) {
+  const size_t es = s.dtype == XG_F32 ? 4 : 8;
+  const int ndim = s.ndim, ax = s.axis, lo = s.pad_lo;
+  const int64_t kept = scan_shape[ax];
+  int64_t out_shape[XG_MAX_NDIM], plane_shape[XG_MAX_NDIM];
+  for (int d = 0; d < ndim; ++d) out_shape[d] = plane_shape[d] = scan_shape[d];
+  out_shape[ax] = kept + s.pad_lo + s.pad_hi;
+  plane_shape[ax] = 1;
+  const View3 vin = view3(ndim, s.shape, 0), vout = view3(ndim, out_shape, 0);
+  const View3 vscan = view3(ndim, scan_shape, 0), vplane = view3(ndim, plane_shape, 0);
+  return spread(who, s.device, vout.L, false, [&](int device, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(device);
+    if (rc) return rc;
+    if (vout.L <= 0 || vout.R == 0) return XG_OK;
+    const void *d_pre, *d_post, *d_fill;
+    rc = ss.upload(kAuxPre, s.pre, s.pre ? operand_span(s.pre_strides, s.shape, ndim, es) : 0, &d_pre);
+    if (rc == XG_OK)
+      rc = ss.upload(kAuxPost, s.post, s.post ? operand_span(s.post_strides, out_shape, ndim, es) : 0, &d_post);
+    if (rc == XG_OK) rc = ss.upload(kAuxFill, fill_host, es, &d_fill);
+    if (rc == XG_OK) rc = ss.fence();
+    if (rc) return rc;
+
+    PipeExtra ex;
+    ex.scratch_row_bytes = (size_t)vscan.R * es;
+    ex.plane_row_bytes = (size_t)vplane.R * es;
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      int64_t sshape[XG_MAX_NDIM], cshape[XG_MAX_NDIM], oshape[XG_MAX_NDIM], pshape[XG_MAX_NDIM];
+      for (int d = 0; d < ndim; ++d) {
+        sshape[d] = s.shape[d];
+        cshape[d] = scan_shape[d];
+        oshape[d] = out_shape[d];
+        pshape[d] = plane_shape[d];
+      }
+      sshape[0] = cshape[0] = oshape[0] = pshape[0] = j1 - j0;
+      const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(j0 * s.pre_strides[0]) * es : nullptr;
+      const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * s.post_strides[0]) * es : nullptr;
+      int rc2 = xg_cumscan(s.dtype, b.in, b.scratch, ndim, sshape, ax, s.reverse, s.trim, 0, 0, XG_BC_NONE, 0.0, pm,
+                           s.pre_strides, nullptr, nullptr, s.skipna, st);
+      if (rc2) return rc2;
+      SlabBufs scanned = b;  // the halo is taken from the scanned slab, as pad() takes it from the scanned field
+      scanned.in = b.scratch;
+      const void *hl = nullptr, *hh = nullptr;
+      rc2 = halo(scanned, cshape, nullptr, d_fill, st, &hl, &hh);
+      if (rc2) return rc2;
+      // the scanned slab at row `lo` of the padded axis, its halo planes at row 0 and row lo + kept
+      int64_t ostr[XG_MAX_NDIM], cstr[XG_MAX_NDIM], pstr[XG_MAX_NDIM];
+      for (int64_t d = ndim - 1, o = 1, c = 1, p = 1; d >= 0; o *= oshape[d], c *= cshape[d], p *= pshape[d], --d) {
+        ostr[d] = o;
+        cstr[d] = c;
+        pstr[d] = p;
+      }
+      char* o = static_cast<char*>(b.out[0]);
+      void* dst[3] = {o + (size_t)(lo * ostr[ax]) * es, nullptr, nullptr};
+      const void* src[3] = {b.scratch, nullptr, nullptr};
+      int64_t shapes[3 * XG_MAX_NDIM], dstr[3 * XG_MAX_NDIM], sstr[3 * XG_MAX_NDIM];  // count x ndim, row-major
+      int neg[3] = {0, 0, 0}, count = 1;
+      for (int d = 0; d < ndim; ++d) {
+        shapes[d] = cshape[d];
+        dstr[d] = ostr[d];
+        sstr[d] = cstr[d];
+      }
+      for (int side = 0; side < 2; ++side) {
+        const void* plane = side ? hh : hl;
+        if (!plane) continue;
+        dst[count] = o + (size_t)((side ? lo + kept : 0) * ostr[ax]) * es;
+        src[count] = plane;
+        for (int d = 0; d < ndim; ++d) {
+          shapes[count * ndim + d] = pshape[d];
+          dstr[count * ndim + d] = ostr[d];
+          sstr[count * ndim + d] = pstr[d];
+        }
+        ++count;
+      }
+      // dense arrays differ in the padded axis alone: every copy collapses to at most 3 dims
+      rc2 = xg_strided_copy_batch(s.dtype, count, dst, src, ndim, shapes, dstr, sstr, neg, st);
+      if (rc2 || !qm) return rc2;
+      return xg_binary(XG_BIN_DIV, s.dtype, o, qm, s.post_strides, o, ndim, oshape, st);
+    };
+    void* outs[1] = {s.out};
+    return ss.run(es, s.in, vin, 1, outs, &vout, launch, ex.rows(r0, r1));
+  });
+}
+
 }  // namespace
 }  // namespace xg_host
 
@@ -662,14 +886,9 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   const std::string who = "xg_stencil2_host_connected";
   const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, (lo || hi) ? XG_BC_FILL : XG_BC_NONE,
                fill_value, nullptr, nullptr, post_metric, post_strides, device};
+  const CopyList cl{ncopies, copy_ndim, side, source, dst_offset, src_offset, shapes, dst_strides, src_strides, negate};
   int rc = validate_halo_call(who.c_str(), c);
   if (rc) return rc;
-  if (ncopies < 0) return xg_fail(XG_EINVAL, who + ": negative copy count");
-  if (ncopies > 0 && (!side || !source || !dst_offset || !src_offset || !shapes || !dst_strides ||
-                      !src_strides || !negate))
-    return xg_fail(XG_EINVAL, who + ": null pointer in the copy list");
-  if (ncopies > 0 && (copy_ndim < 1 || copy_ndim > XG_MAX_NDIM))
-    return xg_fail(XG_EINVAL, who + ": bad copy rank");
   if (partner && !partner_shape) return xg_fail(XG_EINVAL, who + ": null partner shape");
   const int64_t n0 = shape[0];
   int64_t row_in = 1;
@@ -685,75 +904,59 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
       partner_row *= partner_shape[d];
     }
   }
-  int64_t covered[2] = {0, 0};
   bool fill = false;
-  for (int k = 0; k < ncopies; ++k) {
-    const int64_t* sh = shapes + (size_t)k * copy_ndim;
-    const int64_t* ds = dst_strides + (size_t)k * copy_ndim;
-    const int64_t* ss = src_strides + (size_t)k * copy_ndim;
-    const std::string at = who + ": copy " + std::to_string(k) + ": ";
-    if (side[k] != 0 && side[k] != 1) return xg_fail(XG_EINVAL, at + "side must be 0 (lo) or 1 (hi)");
-    if (!(side[k] ? hi : lo)) return xg_fail(XG_EINVAL, at + "writes a halo plane the call does not pad");
-    if (source[k] < kSrcField || source[k] > kSrcFill)
-      return xg_fail(XG_EINVAL, at + "source must be 0 (field), 1 (partner) or 2 (fill constant)");
-    if (source[k] == kSrcPartner && !partner) return xg_fail(XG_EINVAL, at + "reads a partner that was not given");
-    fill = fill || source[k] == kSrcFill;
-    int64_t cells = 1;
-    for (int d = 0; d < copy_ndim; ++d) {
-      if (sh[d] < 0) return xg_fail(XG_EINVAL, at + "negative extent");
-      cells *= sh[d];
-    }
-    covered[side[k]] += cells;
-    const int64_t src_row = source[k] == kSrcField ? row_in : source[k] == kSrcPartner ? partner_row : 0;
-    if (sh[0] != n0 || ds[0] != plane_row || ss[0] != src_row)
-      return xg_fail(XG_EINVAL, at + "must span dim 0 in full with the contiguous dim-0 strides");
-    if (cells == 0) continue;
-    int64_t a, b;
-    copy_extent(dst_offset[k], ds, sh, copy_ndim, &a, &b);
-    if (a < 0 || b >= n0 * plane_row) return xg_fail(XG_EINVAL, at + "leaves the halo plane");
-    copy_extent(src_offset[k], ss, sh, copy_ndim, &a, &b);
-    if (source[k] == kSrcFill) {
-      if (a != 0 || b != 0) return xg_fail(XG_EINVAL, at + "the fill constant is read with offset 0, strides 0");
-    } else if (a < 0 || b >= n0 * src_row) {
-      return xg_fail(XG_EINVAL, at + "leaves its source array");
-    }
-  }
-  // the copies write disjoint cells, so together they must cover each padded plane exactly once
-  if ((lo && covered[0] != n0 * plane_row) || (hi && covered[1] != n0 * plane_row))
-    return xg_fail(XG_EINVAL, who + ": the copies do not cover the halo planes");
-
+  rc = validate_copies(who, cl, lo, hi, n0, plane_row, row_in, partner != nullptr, partner_row, &fill);
+  if (rc) return rc;
   const size_t es = dtype == XG_F32 ? 4 : 8;
   const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
   const void* fill_host = fill ? (es == 4 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
-  // the whole-field copy list rebased onto each slab's buffers, `rows` high.  The rebased pointers and shapes are
-  // built per slab, on every path (three vectors of ncopies entries, small beside a slab's copies): the stage then
-  // keeps no state between slabs, so the members of a host device group can run it at once.
-  auto copies = [&](const SlabBufs& b, const int64_t* slab_shape, const void*, const void* d_fill, cudaStream_t st,
-                    const void** hl, const void** hh) -> int {
-    std::vector<void*> dptr(ncopies);
-    std::vector<const void*> sptr(ncopies);
-    std::vector<int64_t> shp(shapes ? shapes : (const int64_t*)nullptr,
-                             shapes ? shapes + (size_t)ncopies * copy_ndim : (const int64_t*)nullptr);
-    for (int k = 0; k < ncopies; ++k) {
-      dptr[k] = static_cast<char*>(b.plane[side[k]]) + (size_t)dst_offset[k] * es;
-      const void* base = source[k] == kSrcField ? b.in : source[k] == kSrcPartner ? b.in2 : d_fill;
-      sptr[k] = static_cast<const char*>(base) + (size_t)src_offset[k] * es;
-      shp[(size_t)k * copy_ndim] = slab_shape[0];
-    }
-    if (lo) *hl = b.plane[0];
-    if (hi) *hh = b.plane[1];
-    int rc2 = xg_strided_copy_batch(dtype, ncopies, dptr.data(), sptr.data(), copy_ndim, shp.data(), dst_strides,
-                                    src_strides, negate, st);
-    if (rc2 != XG_ENOTIMPL) return rc2;
-    for (int k = 0; k < ncopies; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
-      rc2 = xg_strided_copy(dtype, dptr[k], dst_strides + (size_t)k * copy_ndim, sptr[k],
-                            src_strides + (size_t)k * copy_ndim, copy_ndim, shp.data() + (size_t)k * copy_ndim,
-                            negate[k], st);
-      if (rc2) return rc2;
-    }
-    return XG_OK;
-  };
-  return stencil_host(who.c_str(), c, nullptr, partner, partner_row, copies, fill_host);
+  return stencil_host(who.c_str(), c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
+                      fill_host);
+}
+
+extern "C" int xg_cumscan_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,
+                                    int reverse, int trim, int pad_lo, int pad_hi, const void* pre_metric,
+                                    const int64_t* pre_strides, const void* post_metric, const int64_t* post_strides,
+                                    int skipna, int seam_axis, int skip, int64_t mirror, int64_t period, int device) {
+  const char* who = "xg_cumscan_host_fold";
+  const ScanCall s{dtype, in, out, ndim, shape, axis, reverse, trim, pad_lo, pad_hi,
+                   pre_metric, pre_strides, post_metric, post_strides, skipna, device};
+  int64_t scan_shape[XG_MAX_NDIM];
+  int rc = validate_scan_call(who, s, scan_shape);
+  if (rc) return rc;
+  if (pad_lo != 0 || pad_hi != 1)
+    return xg_fail(XG_EINVAL, std::string(who) + ": the fold pads the north edge alone: pad_lo must be 0, pad_hi 1");
+  // the fold row of the scanned field: its own rows and skip, no weight
+  const Call c{0, dtype, in, out, ndim, scan_shape, axis, 0, 1, XG_BC_NONE, 0.0, nullptr, nullptr, nullptr, nullptr,
+               device};
+  rc = validate_fold(who, c, seam_axis, skip, mirror, period);
+  return rc ? rc
+            : cumscan_halo_host(who, s, scan_shape, fold_stage(c, false, seam_axis, skip, mirror, period, 0), nullptr);
+}
+
+extern "C" int xg_cumscan_host_connected(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                         int axis, int reverse, int trim, int pad_lo, int pad_hi, double fill_value,
+                                         const void* pre_metric, const int64_t* pre_strides, const void* post_metric,
+                                         const int64_t* post_strides, int skipna, int ncopies, int copy_ndim,
+                                         const int* side, const int* source, const int64_t* dst_offset,
+                                         const int64_t* src_offset, const int64_t* shapes, const int64_t* dst_strides,
+                                         const int64_t* src_strides, const int* negate, int device) {
+  const char* who = "xg_cumscan_host_connected";
+  const ScanCall s{dtype, in, out, ndim, shape, axis, reverse, trim, pad_lo, pad_hi,
+                   pre_metric, pre_strides, post_metric, post_strides, skipna, device};
+  const CopyList cl{ncopies, copy_ndim, side, source, dst_offset, src_offset, shapes, dst_strides, src_strides, negate};
+  int64_t scan_shape[XG_MAX_NDIM];
+  int rc = validate_scan_call(who, s, scan_shape);
+  if (rc) return rc;
+  // the copies read the scanned field
+  int64_t row = 1;
+  for (int d = 1; d < ndim; ++d) row *= scan_shape[d];
+  bool fill = false;
+  rc = validate_copies(who, cl, pad_lo, pad_hi, scan_shape[0], row / scan_shape[axis], row, false, 0, &fill);
+  if (rc) return rc;
+  const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
+  const void* fill_host = fill ? (dtype == XG_F32 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
+  return cumscan_halo_host(who, s, scan_shape, copy_stage(cl, dtype, pad_lo, pad_hi), fill_host);
 }
 
 extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,

@@ -46,7 +46,12 @@ from .grid_ufunc import (
 )
 from .labeled import DataArray, Dataset, is_device_array
 from .metrics import iterate_axis_combinations
-from .padding import fold_edges, pad  # noqa: F401  (pad: re-exported like the reference's grid module)
+from .padding import (  # noqa: F401  (pad: re-exported like the reference's grid module)
+    _get_all_connection_axes,
+    connected_edge_mode,
+    fold_edges,
+    pad,
+)
 
 
 def _maybe_promote_str_to_list(a):
@@ -975,16 +980,19 @@ class Grid:
         fills = self._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
 
         host_input = not da.is_device
-        # numpy-backed field, one axis: stream slabs through the GPU (xg_cumscan_host) instead of one
-        # un-overlapped upload + download around the kernel
-        host_stream = (host_input and len(axis) == 1 and self._face_connections is None
-                       and np.asarray(da.data).dtype in (np.float32, np.float64)
-                       and axis[0] not in self._folds)  # (the slab pipeline takes no fold halo)
-        if host_stream:
-            data = da
-        else:
-            x, _ = as_device_tensor(da.data, self._device_for(da))
-            data = da._replace(data=x)
+        # numpy-backed field, one axis: stream slabs through the GPU (xg_cumscan_host, or its _fold / _connected
+        # twin where the padded edge crosses a north fold or a face connection) instead of one un-overlapped
+        # upload + download around the kernel
+        host_stream = (host_input and len(axis) == 1
+                       and np.asarray(da.data).dtype in (np.float32, np.float64))
+        data = da
+
+        def to_device(data):
+            x, _ = as_device_tensor(data.data, self._device_for(da))
+            return data._replace(data=x)
+
+        if not host_stream:
+            data = to_device(data)
         for ax_i, ax_name in enumerate(axis):
             ax = self.axes[ax_name]
             pos, dim = ax._get_position_name(da)
@@ -1016,6 +1024,24 @@ class Grid:
             pre_t = post_t = None
             probe = DataArray.__new__(DataArray)
             probe._dims = out_dims
+            fv = fills[ax.name] if fills[ax.name] is not None else 0.0
+            bc = ax_padding if (pad_lo or pad_hi) else None
+            halo = None  # the fold or face connection a streamed call's padded edge crosses
+            if host_stream and (self._face_connections is not None or ax.name in self._folds):
+                if weighted and _pre_weight is not None:
+                    host_stream = False  # not streamed (below), but works on the whole-field route
+                elif self._face_connections is not None and (pad_lo or pad_hi):
+                    if paddings[ax.name] not in (None, "periodic", "fill", "extend"):
+                        host_stream = False  # e.g. a per-side mapping: pad() has the say
+                    elif ax.name in _get_all_connection_axes(self._face_connections, self._facedim):
+                        halo = "connected"
+                    else:  # e.g. Z on LLC: the basic boundary, checked as pad() checks it
+                        bc, fv = connected_edge_mode(self, ax.name, pad_lo, pad_hi, padding, fill_value,
+                                                     data.sizes[self._facedim])
+                elif folded:
+                    halo = "fold"
+                if not host_stream:
+                    data = to_device(data)
             if host_stream:
                 fdt = np.asarray(data.data).dtype
                 if weighted:
@@ -1025,7 +1051,15 @@ class Grid:
                     if pre_t is not None:
                         raise NotImplementedError("cumint with metric_weighted on a host array: pass a device array")
                     pre_t = self._metric_host(_pre_weight, data.dims, fdt)
-            else:
+                if halo is not None:
+                    y = _cumsum_halo_host(self, halo, np.asarray(data.data), data.dims, ax.name, dim, ax_reverse,
+                                          trim, pad_lo, pad_hi, padding, fill_value, pre_t, post_t,
+                                          self._host_device(da))
+                    if y is None:  # a layout that does not stream
+                        host_stream = False
+                        pre_t = post_t = None
+                        data = to_device(data)
+            if not host_stream:
                 if weighted:
                     pre_t = self._metric_tensor(self.get_metric(data, weighted), data.dims, data.data)
                     post_t = self._metric_tensor(self.get_metric(probe, weighted), out_dims, data.data)
@@ -1035,8 +1069,11 @@ class Grid:
                         pre_t = w_t  # (da * w) is formed inside the scan kernel: 8 B/cell instead of 20
                     else:  # two roundings in the reference, (da * w) * metric: keep them
                         data = data._replace(data=ops.binary("mul", data.data, w_t))
-            fv = fills[ax.name] if fills[ax.name] is not None else 0.0
-            if (self._face_connections is not None and (pad_lo or pad_hi)) or folded:
+            if host_stream:
+                if halo is None:
+                    y = ops.cumscan_host(np.asarray(data.data), axis_num, ax_reverse, trim, pad_lo, pad_hi, bc, fv,
+                                         pre=pre_t, post=post_t, skipna=True, device=self._host_device(da))
+            elif (self._face_connections is not None and (pad_lo or pad_hi)) or folded:
                 # the reference pads the cumsum'd data with ``pad`` (grid.py:1385-1391), which on a
                 # connected grid takes the halo from the neighbour face and across a north fold
                 # mirrors the scanned rows: scan + trim in the kernel, halo through ``pad``, metric
@@ -1048,17 +1085,9 @@ class Grid:
                         fill_value=fill_value).data
                 if post_t is not None:
                     y = ops.binary("div", y, post_t)
-            elif host_stream:
-                y = ops.cumscan_host(
-                    np.asarray(data.data), axis_num, ax_reverse, trim, pad_lo, pad_hi,
-                    ax_padding if (pad_lo or pad_hi) else None, fv, pre=pre_t, post=post_t, skipna=True,
-                    device=self._host_device(da),
-                )
             else:
-                y = ops.cumscan(
-                    data.data, axis_num, ax_reverse, trim, pad_lo, pad_hi,
-                    ax_padding if (pad_lo or pad_hi) else None, fv, pre=pre_t, post=post_t, skipna=True,
-                )
+                y = ops.cumscan(data.data, axis_num, ax_reverse, trim, pad_lo, pad_hi, bc, fv, pre=pre_t,
+                                post=post_t, skipna=True)
             coordless = DataArray(y, dims=out_dims, name=da.name, attrs=da.attrs)
             data = _reattach_coords(
                 [coordless], grid=self, padding_width={ax.name: (pad_lo, pad_hi)},
@@ -1224,6 +1253,54 @@ class Grid:
 
 # (from, to) -> (trim, (pad_lo, pad_hi)); transcription of the enumerated shifts of
 # reference grid.py:1326-1383
+def _cumsum_halo_host(grid, kind, x, dims, ax_name, dim, reverse, trim, pad_lo, pad_hi, padding, fill_value, pre,
+                      post, device):
+    """One axis of ``Grid.cumsum`` on the numpy field ``x`` whose padded edge crosses a north fold (``kind``
+    "fold") or a face connection ("connected"), streamed in slabs by ``xg_cumscan_host_fold`` /
+    ``_connected``: per slab the device route's scan, halo of the scanned field (as ``pad`` builds it) and
+    divide by ``post``.  The slabs are cut as the stencils cut them (``grid_ufunc._host_stream_route``); the
+    halo is planned for the scanned, merged layout.  Returns the result, or None when the layout does not stream
+    (no batch dim in front, or a fold the plan cannot mirror): the whole-field route then runs."""
+    from . import ops
+    from .grid_ufunc import _host_stream_route, _merge_leading
+    from .padding import _axis_dim, _fold_plan, connected_halo_program
+
+    dims = tuple(dims)
+    shape = [int(v) for v in x.shape]
+    axis_num = dims.index(dim)
+    if kind == "fold":
+        core = [dim, _axis_dim(grid, dims, grid._folds[ax_name]["seam_axis"])]
+    else:
+        core = [dim, grid._facedim] + [d for a in _get_all_connection_axes(grid._face_connections, grid._facedim)
+                                       for d in grid.axes[a].coords.values() if d in dims]
+    route = _host_stream_route(kind, dims, shape, core, pad_lo, pad_hi,
+                               operand_shapes=[m.shape for m in (pre, post) if m is not None])
+    if route is None:
+        return None
+    _, ndrop, nmerge = route
+    lead = ndrop + nmerge
+    cut = lambda a: None if a is None else _merge_leading(a, ndrop, nmerge)  # noqa: E731
+    m_dims = dims[ndrop:ndrop + 1] + dims[lead:]  # the merged batch dim keeps the name of its first dim
+    scanned = list(shape)
+    scanned[axis_num] -= 0 if trim == "none" else 1
+    m_scanned = [int(np.prod(scanned[ndrop:lead]))] + scanned[lead:]
+    ax = axis_num - lead + 1
+    kw = dict(pre=cut(pre), post=cut(post), skipna=True, device=device)
+    if kind == "fold":
+        try:
+            _, seam, skip, mirror, period = _fold_plan(grid, ax_name, m_dims, m_scanned, 1)
+        except NotImplementedError:
+            return None
+        out = ops.cumscan_host_fold(cut(x), ax, reverse, trim, seam, skip, mirror, period, **kw)
+    else:
+        mode, fv = connected_edge_mode(grid, ax_name, pad_lo, pad_hi, padding, fill_value,
+                                       shape[dims.index(grid._facedim)])
+        program = connected_halo_program(grid, ax_name, pad_lo, pad_hi, m_dims, m_scanned, mode)
+        out = ops.cumscan_host_connected(cut(x), ax, reverse, trim, pad_lo, pad_hi, fv, program, **kw)
+    scanned[axis_num] += pad_lo + pad_hi
+    return out.reshape(scanned)
+
+
 _CUMSUM_FWD = {
     ("center", "right"): ("none", (0, 0)),
     ("left", "center"): ("none", (0, 0)),

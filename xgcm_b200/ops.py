@@ -643,6 +643,22 @@ def stencil2_host_fold(x: np.ndarray, axis: int, op: str, lo: int, hi: int, padd
 _HALO_SOURCES = {"self": 0, "partner": 1, "fill": 2}
 
 
+def _copy_list_args(program: Sequence[tuple]):
+    """C-ABI arguments of a face-connection copy list (``padding.connected_halo_program``): count, rank, sides,
+    sources, dst / src offsets, then the flattened shapes, dst strides, src strides and the negate flags."""
+    import ctypes as C
+
+    n = len(program)
+    cndim = len(program[0][6]) if n else 1
+    if any(len(c[6]) != cndim or len(c[2]) != cndim or len(c[5]) != cndim for c in program):
+        raise ValueError("every copy of a halo program must have the same rank")
+    i32 = lambda vals: (C.c_int * max(n, 1))(*vals)  # noqa: E731
+    flat = lambda k: _capi.i64_array([int(v) for c in program for v in c[k]] or [0])  # noqa: E731
+    return (n, cndim, i32([int(c[0]) for c in program]), i32([_HALO_SOURCES[c[3]] for c in program]),
+            _capi.i64_array([int(c[1]) for c in program] or [0]), _capi.i64_array([int(c[4]) for c in program] or [0]),
+            flat(6), flat(2), flat(5), i32([1 if c[7] else 0 for c in program]))
+
+
 def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int, fill_value: float,
                             program: Sequence[tuple], partner: Optional[np.ndarray] = None,
                             post: Optional[np.ndarray] = None, out: Optional[np.ndarray] = None,
@@ -652,8 +668,6 @@ def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int,
     ``padding.connected_halo_program`` — ``(side, dst offset, dst strides, source ("self", "partner" or
     "fill"), src offset, src strides, shape, negate)`` for the whole field, clipped to each slab by the
     library.  ``partner`` (the other vector component) streams beside ``x``; "fill" reads ``fill_value``."""
-    import ctypes as C
-
     lib = _capi.load()
     x, shape, axis, out, _, post_op, dev = _host_stencil_prep(x, axis, op, lo, hi, "fill" if (lo or hi) else None,
                                                               None, post, out, device, "stencil2_host_connected")
@@ -663,19 +677,12 @@ def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int,
         p_shape = list(partner.shape)
         if len(p_shape) != x.ndim:
             raise ValueError(f"partner component of shape {tuple(p_shape)} has not the rank of the field {tuple(shape)}")
-    n = len(program)
-    cndim = len(program[0][6]) if n else 1
-    if any(len(c[6]) != cndim or len(c[2]) != cndim or len(c[5]) != cndim for c in program):
-        raise ValueError("stencil2_host_connected: every copy must have the same rank")
-    i32 = lambda vals: (C.c_int * max(n, 1))(*vals)  # noqa: E731
-    flat = lambda k: _capi.i64_array([int(v) for c in program for v in c[k]] or [0])  # noqa: E731
+    n, cndim, side, source, doff, soff, shapes, dstr, sstr, neg = _copy_list_args(program)
     rc = lib.xg_stencil2_host_connected(
         _capi.OPS[op], _capi.dtype_code(x.dtype), x.ctypes.data,
         None if partner is None else partner.ctypes.data, _capi.i64_array(p_shape), out.ctypes.data, x.ndim,
-        _capi.i64_array(shape), axis, lo, hi, float(fill_value), post_op[1], post_op[2], n, cndim,
-        i32([int(c[0]) for c in program]), i32([_HALO_SOURCES[c[3]] for c in program]),
-        _capi.i64_array([int(c[1]) for c in program] or [0]), _capi.i64_array([int(c[4]) for c in program] or [0]),
-        flat(6), flat(2), flat(5), i32([1 if c[7] else 0 for c in program]), dev,
+        _capi.i64_array(shape), axis, lo, hi, float(fill_value), post_op[1], post_op[2], n, cndim, side, source,
+        doff, soff, shapes, dstr, sstr, neg, dev,
     )
     _capi.check(rc)
     return out
@@ -902,9 +909,22 @@ def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "n
                  device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`cumscan` (``xg_cumscan_host``): slabs of a non-operated dim stream through the GPU."""
     lib = _capi.load()
-    x = _host_field(x, "field")
     if padding not in _capi.BCS:
         raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}")
+    x, shape, axis, out, pre_op, post_op, dev = _host_scan_prep(x, axis, trim, pad_lo, pad_hi, pre, post, device)
+    if out.size:
+        rc = lib.xg_cumscan_host(
+            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), axis,
+            int(bool(reverse)), _capi.TRIMS[trim], pad_lo, pad_hi, _capi.BCS[padding], float(fill_value),
+            pre_op[1], pre_op[2], post_op[1], post_op[2], int(bool(skipna)), dev)
+        _capi.check(rc)
+    return out
+
+
+def _host_scan_prep(x, axis, trim, pad_lo, pad_hi, pre, post, device):
+    """Checks and buffers shared by the host cumscan twins: (contiguous x, shape, axis, out, pre operand, post
+    operand, device index)."""
+    x = _host_field(x, "field")
     axis = _norm_axis(axis, x.ndim)
     shape = list(x.shape)
     kept = shape[axis] - (0 if trim == "none" else 1)
@@ -913,14 +933,46 @@ def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "n
     out_shape = list(shape)
     out_shape[axis] = kept + pad_lo + pad_hi
     out = pinned_empty(out_shape, x.dtype)
-    kp, pre_ptr, pre_st = _host_operand(pre, shape, x.dtype, "pre metric")
-    kq, post_ptr, post_st = _host_operand(post, out_shape, x.dtype, "post metric")
-    dev = host_device_arg(device)
+    pre_op = _host_operand(pre, shape, x.dtype, "pre metric")
+    post_op = _host_operand(post, out_shape, x.dtype, "post metric")
+    return x, shape, axis, out, pre_op, post_op, host_device_arg(device)
+
+
+def cumscan_host_fold(x: np.ndarray, axis: int, reverse: bool, trim: str, seam_axis: int, skip: int, mirror: int,
+                      period: int, pre: Optional[np.ndarray] = None, post: Optional[np.ndarray] = None,
+                      skipna: bool = True, device: HostDevice = None) -> np.ndarray:
+    """:func:`cumscan_host` whose north edge is padded across a fold (``xg_cumscan_host_fold``): bit for bit
+    :func:`cumscan` (``pre``, no post), then the folded row of the scanned field as one row above it
+    (:func:`fold_rows` with ``seam_axis, skip, mirror, period``, planned for the scanned shape), then ``/ post``.
+    Dim 0 is cut into slabs and must be neither ``axis`` nor ``seam_axis``."""
+    lib = _capi.load()
+    x, shape, axis, out, pre_op, post_op, dev = _host_scan_prep(x, axis, trim, 0, 1, pre, post, device)
     if out.size:
-        rc = lib.xg_cumscan_host(
+        rc = lib.xg_cumscan_host_fold(
             _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), axis,
-            int(bool(reverse)), _capi.TRIMS[trim], pad_lo, pad_hi, _capi.BCS[padding], float(fill_value),
-            pre_ptr, pre_st, post_ptr, post_st, int(bool(skipna)), dev)
+            int(bool(reverse)), _capi.TRIMS[trim], 0, 1, pre_op[1], pre_op[2], post_op[1], post_op[2],
+            int(bool(skipna)), _norm_axis(seam_axis, x.ndim), int(skip), int(mirror), int(period), dev)
+        _capi.check(rc)
+    return out
+
+
+def cumscan_host_connected(x: np.ndarray, axis: int, reverse: bool, trim: str, pad_lo: int, pad_hi: int,
+                           fill_value: float, program: Sequence[tuple], pre: Optional[np.ndarray] = None,
+                           post: Optional[np.ndarray] = None, skipna: bool = True,
+                           device: HostDevice = None) -> np.ndarray:
+    """:func:`cumscan_host` on a grid with face connections (``xg_cumscan_host_connected``): bit for bit
+    :func:`cumscan` (``pre``, no post), then the halo planes written by ``program`` — the copy list of
+    :func:`stencil2_host_connected`, built by ``padding.connected_halo_program`` for the SCANNED field's shape,
+    sources "self" and "fill" — then ``/ post``."""
+    lib = _capi.load()
+    x, shape, axis, out, pre_op, post_op, dev = _host_scan_prep(x, axis, trim, pad_lo, pad_hi, pre, post, device)
+    if out.size:
+        n, cndim, side, source, doff, soff, shapes, dstr, sstr, neg = _copy_list_args(program)
+        rc = lib.xg_cumscan_host_connected(
+            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), axis,
+            int(bool(reverse)), _capi.TRIMS[trim], pad_lo, pad_hi, float(fill_value), pre_op[1], pre_op[2],
+            post_op[1], post_op[2], int(bool(skipna)), n, cndim, side, source, doff, soff, shapes, dstr, sstr, neg,
+            dev)
         _capi.check(rc)
     return out
 
