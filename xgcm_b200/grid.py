@@ -30,7 +30,7 @@ import inspect
 import itertools
 import warnings
 from collections import OrderedDict
-from typing import Any, Callable, Dict, Iterable, List, Mapping, Optional, Sequence, Tuple, Union
+from typing import Any, Callable, Dict, Iterable, List, Mapping, NamedTuple, Optional, Sequence, Tuple, Union
 
 import numpy as np
 
@@ -40,8 +40,11 @@ from .grid_ufunc import (
     GridUFunc,
     _check_data_input,
     _GridUFuncSignature,
+    _host_stream_route,
+    _is_host_float,
     _maybe_unpack_vector_component,
     _reattach_coords,
+    _stencil_boundary,
     apply_as_grid_ufunc,
 )
 from .labeled import DataArray, Dataset, is_device_array
@@ -50,6 +53,7 @@ from .padding import (  # noqa: F401  (pad: re-exported like the reference's gri
     _get_all_connection_axes,
     connected_edge_mode,
     fold_edges,
+    missing_boundary_error,
     pad,
 )
 
@@ -568,7 +572,7 @@ class Grid:
             and not isinstance(data, dict)
             and set(kwargs) <= {"padding", "fill_value"}
         ):
-            fused = self._fused_multi_axis(funcname, array, axis, signatures, kwargs)
+            fused = self._fused_multi_axis(funcname, array, axis, to, kwargs)
             if fused is not None:
                 return self._wrap_out(fused, as_xarray)
         if host_input and n_axes > 1:
@@ -600,7 +604,7 @@ class Grid:
             array = array._replace(data=result_like(array.data, True))
         return self._wrap_out(array, as_xarray)
 
-    def _fused_multi_axis(self, funcname, array, axis, signatures, kwargs):
+    def _fused_multi_axis(self, funcname, array, axis, to, kwargs):
         """All axes of a multi-axis diff / interp / min / max in ONE kernel launch
         (``xg_stencil_multi``): same values as the per-axis loop of grid.py:800-832, one read and
         one write of the field instead of one pass per axis.  Returns None when the fused kernel
@@ -613,38 +617,19 @@ class Grid:
         paddings = self._complete_user_kwargs_using_axis_defaults(kwargs.get("padding"), "padding")
         fills = self._complete_user_kwargs_using_axis_defaults(kwargs.get("fill_value"), "fill_value")
         specs, rename = [], {}
-        for sig, ax_name in zip(signatures, axis):
-            grid_ufunc, _ = _select_grid_ufunc(funcname, sig, module=gridops)
-            dummy = grid_ufunc.signature.in_ax_names[0][0]  # the ufunc's own dummy axis name ("X")
-            lo, hi = (grid_ufunc.padding_width or {}).get(dummy, (0, 0))
-            from_pos = sig.in_ax_positions[0][0]
-            to_pos = sig.out_ax_positions[0][0]
-            in_dim = self.axes[ax_name].coords[from_pos]
-            try:
-                out_dim = self.axes[ax_name].coords[to_pos]
-            except KeyError:
-                raise ValueError(f"Axis position ({ax_name}:{to_pos}) does not exist in grid")
-            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
-            if folded:
+        for ax_name in axis:
+            t = _stencil_term(self, funcname, array, ax_name, to.get(ax_name), paddings, fills)
+            if t.folded:
                 return None  # the fold row is a halo plane of the per-axis launch
-            if (lo or hi) and pad_mode is None:
-                raise ValueError(
-                    f"No boundary condition was specified for axis {ax_name!r}, but the "
-                    f"requested operation needs to pad it. Set a boundary condition, "
-                    f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                    f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                    f"grid method."
-                )
-            if pad_mode not in ("periodic", "fill", "extend", None):
+            if t.pad_mode not in ("periodic", "fill", "extend", None):
                 return None  # e.g. the opt-in extrapolate extension: per-axis path
-            fv = fills[ax_name] if fills[ax_name] is not None else 0.0
-            specs.append((array.get_axis_num(in_dim), funcname, lo, hi, pad_mode if (lo or hi) else None, fv))
-            rename[in_dim] = out_dim
+            specs.append((t.axis_num, funcname, t.lo, t.hi, t.pad_mode if (t.lo or t.hi) else None, t.fill))
+            rename[t.in_dim] = t.out_dim
         if array.shape[-1] < 32:
             return None  # tiny rows: the one-block-per-row kernel has nothing to chew on
         out = None
         dev = self._device_for(array)
-        if not array.is_device and dev.type == "cuda" and np.asarray(array.data).dtype in (np.float32, np.float64):
+        if _is_host_float(array) and dev.type == "cuda":
             # numpy-backed field: slabs stream through the GPU (xg_stencil_multi_host), so input, result and the
             # device footprint need not fit in HBM together
             try:
@@ -689,43 +674,24 @@ class Grid:
             return [self._wrap_out(self._1d_grid_ufunc_dispatch(f, da, a, to=t, **kw), as_xarray)
                     for f, a, t in reqs]
 
-        host_ok = (not isinstance(da, dict) and not da.is_device and self._face_connections is None
-                   and np.asarray(da.data).dtype in (np.float32, np.float64) and 1 <= len(reqs) <= 8)
+        host_ok = (not isinstance(da, dict) and _is_host_float(da) and self._face_connections is None
+                   and 1 <= len(reqs) <= 8)
         if not host_ok:
             return one_by_one()
         paddings = self._complete_user_kwargs_using_axis_defaults(padding, "padding")
         fills = self._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
         specs, renames = [], []
         for funcname, ax_name, to in reqs:
-            sig = self._create_1d_grid_ufunc_signatures(da, axis=[ax_name], to=self._map_kwargs_over_axes(to))[0]
-            grid_ufunc, _ = _select_grid_ufunc(funcname, sig, module=gridops)
-            dummy = grid_ufunc.signature.in_ax_names[0][0]
-            lo, hi = (grid_ufunc.padding_width or {}).get(dummy, (0, 0))
-            from_pos, to_pos = sig.in_ax_positions[0][0], sig.out_ax_positions[0][0]
-            in_dim = self.axes[ax_name].coords[from_pos]
-            try:
-                out_dim = self.axes[ax_name].coords[to_pos]
-            except KeyError:
-                raise ValueError(f"Axis position ({ax_name}:{to_pos}) does not exist in grid")
-            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
-            if folded:
+            t = _stencil_term(self, funcname, da, ax_name, self._map_kwargs_over_axes(to).get(ax_name), paddings,
+                              fills)
+            if t.folded:
                 return one_by_one()  # the host pipeline takes no halo planes
-            if (lo or hi) and pad_mode is None:
-                raise ValueError(
-                    f"No boundary condition was specified for axis {ax_name!r}, but the "
-                    f"requested operation needs to pad it. Set a boundary condition, "
-                    f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                    f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                    f"grid method."
-                )
-            if pad_mode not in ("periodic", "fill", "extend", None):
+            if t.pad_mode not in ("periodic", "fill", "extend", None):
                 return one_by_one()
-            axn = da.get_axis_num(in_dim)
-            if axn == 0 and (lo + hi != 1):
+            if t.axis_num == 0 and (t.lo + t.hi != 1):
                 return one_by_one()  # outer / inner shift along the slab dimension
-            fv = fills[ax_name] if fills[ax_name] is not None else 0.0
-            specs.append((axn, funcname, lo, hi, pad_mode if (lo or hi) else None, fv))
-            renames.append((in_dim, out_dim, ax_name, (lo, hi)))
+            specs.append((t.axis_num, funcname, t.lo, t.hi, t.pad_mode if (t.lo or t.hi) else None, t.fill))
+            renames.append((t.in_dim, t.out_dim, ax_name, (t.lo, t.hi)))
         outs = ops.stencil2_host_multi(np.asarray(da.data), specs, device=self._host_device(da))
         results = []
         for arr, (in_dim, out_dim, ax_name, width) in zip(outs, renames):
@@ -755,7 +721,6 @@ class Grid:
         the operated (and seam) dims stream through the GPU in slabs (``xg_stencil_pair_host``)."""
         from . import ops
         from .device import as_device_tensor, result_like
-        from .grid_ufunc import _host_stream_route, _is_host_float, _merge_leading
         from .padding import _axis_dim, _fold_plan, fold_halo_planes
 
         if combine not in ("add", "sub"):
@@ -800,30 +765,24 @@ class Grid:
         for funcname, da, ax_name in ((funcname_a, da_a, axis_a), (funcname_b, da_b, axis_b)):
             if funcname not in ("diff", "interp", "min", "max") or ax_name not in self.axes:
                 return chain()
-            sig = self._create_1d_grid_ufunc_signatures(da, axis=[ax_name], to={ax_name: to.get(ax_name)})[0]
-            grid_ufunc, _ = _select_grid_ufunc(funcname, sig, module=gridops)
-            dummy = grid_ufunc.signature.in_ax_names[0][0]
-            lo, hi = (grid_ufunc.padding_width or {}).get(dummy, (0, 0))
-            from_pos, to_pos = sig.in_ax_positions[0][0], sig.out_ax_positions[0][0]
-            in_dim = self.axes[ax_name].coords[from_pos]
-            out_dim = self.axes[ax_name].coords.get(to_pos)
-            folded, pad_mode = fold_edges(self, ax_name, paddings[ax_name], hi)
-            if out_dim is None or lo + hi != 1 or pad_mode not in ("periodic", "fill", "extend"):
+            try:
+                t = _stencil_term(self, funcname, da, ax_name, to.get(ax_name), paddings, fills)
+            except ValueError:
+                return chain()  # no such position, or no boundary condition: the chain raises its own error
+            if t.lo + t.hi != 1 or t.pad_mode not in ("periodic", "fill", "extend"):
                 return chain()
-            fv = fills[ax_name] if fills[ax_name] is not None else 0.0
-            terms.append(dict(op=funcname, lo=lo, hi=hi, pad=pad_mode, fill=fv, axn=da.get_axis_num(in_dim),
-                              in_dim=in_dim, out_dim=out_dim, ax=ax_name, folded=folded))
+            terms.append(t)
         ta, tb = terms
-        out_dims_a = tuple(ta["out_dim"] if d == ta["in_dim"] else d for d in da_a.dims)
-        out_dims_b = tuple(tb["out_dim"] if d == tb["in_dim"] else d for d in da_b.dims)
+        out_dims_a = tuple(ta.out_dim if d == ta.in_dim else d for d in da_a.dims)
+        out_dims_b = tuple(tb.out_dim if d == tb.in_dim else d for d in da_b.dims)
         # each term leaves the other's operated dim untouched: the sum needs both to land on the same dims
         if out_dims_a != out_dims_b:
             raise ValueError(f"the two terms land on different positions: {out_dims_a} vs {out_dims_b}")
         last = da_a.ndim - 1
-        if ta["axn"] == last and tb["axn"] != last:
+        if ta.axis_num == last and tb.axis_num != last:
             first, second, fa, fb, ma_ax, mb_ax = ta, tb, da_a, da_b, metric_a, metric_b
             sub = 0 if combine == "add" else 1
-        elif tb["axn"] == last and ta["axn"] != last:
+        elif tb.axis_num == last and ta.axis_num != last:
             first, second, fa, fb, ma_ax, mb_ax = tb, ta, da_b, da_a, metric_b, metric_a
             sub = 0 if combine == "add" else 2  # kernel: innermost term first; we want (a - b) = strided - innermost
         else:
@@ -832,17 +791,17 @@ class Grid:
         dev = self._device_for(da_a)
         # the kernel takes halo planes for the term along the strided dim only; the fold plane and the host twins
         # are CUDA launches (as in grid_ufunc._apply_fused_stencil, a fold off a CUDA device keeps the chain)
-        if first["folded"] or (second["folded"] and dev.type != "cuda"):
+        if first.folded or (second.folded and dev.type != "cuda"):
             return chain()
-        spec_a = (first["op"], first["lo"], first["hi"], first["pad"], first["fill"])
-        spec_b = (second["axn"], second["op"], second["lo"], second["hi"], second["pad"], second["fill"])
+        spec_a = (first.op, first.lo, first.hi, first.pad_mode, first.fill)
+        spec_b = (second.axis_num, second.op, second.lo, second.hi, second.pad_mode, second.fill)
         negate = _components is not None  # a vector component changes sign across the fold
         probe = DataArray.__new__(DataArray)
         probe._dims = out_dims_a
 
         def finish(data):
             res = DataArray(data, dims=out_dims_a, name=da_a.name)
-            res = _reattach_coords([res], self, None, {ta["out_dim"], tb["out_dim"]}, [da_a, da_b])[0]
+            res = _reattach_coords([res], self, None, {ta.out_dim, tb.out_dim}, [da_a, da_b])[0]
             return self._wrap_out(res, as_xarray)
 
         if host and dev.type == "cuda" and _is_host_float(fa) and _is_host_float(fb) and fa.data.dtype == fb.data.dtype:
@@ -851,26 +810,20 @@ class Grid:
             pre_a = self._metric_host(self.get_metric(fa, ma_ax), fa.dims, dt) if ma_ax else None
             pre_b = self._metric_host(self.get_metric(fb, mb_ax), fb.dims, dt) if mb_ax else None
             post = self._metric_host(self.get_metric(probe, divide_by), out_dims_a, dt) if divide_by else None
-            core = [second["in_dim"], dims[-1]]
-            if second["folded"]:
-                core.append(_axis_dim(self, dims, self._folds[second["ax"]]["seam_axis"]))
-            route = _host_stream_route("pair", dims, shape, core, 0, 1,
-                                       operand_shapes=[m.shape for m in (pre_a, pre_b, post) if m is not None])
-            if route is not None:
-                _, ndrop, nmerge = route
-                shift = ndrop + nmerge - 1  # dims before the operated ones that the cut removes
-
-                def cut(a):
-                    return None if a is None else _merge_leading(a, ndrop, nmerge)
-
-                kw = dict(pre_a=cut(pre_a), pre_b=cut(pre_b), post=cut(post), device=self._host_device(da_a))
-                spec_b = (spec_b[0] - shift,) + spec_b[1:]
-                if second["folded"]:
-                    _, seam, skip, mirror, period = _fold_plan(self, second["ax"], dims, shape, 1)
-                    y = ops.stencil_pair_host_fold(cut(fa.data), cut(fb.data), spec_a, spec_b, seam - shift, skip,
-                                                   mirror, period, sub, negate=negate, **kw)
+            core = [second.in_dim, dims[-1]]
+            if second.folded:
+                core.append(_axis_dim(self, dims, self._folds[second.ax_name]["seam_axis"]))
+            cut = _host_stream_route("pair", dims, shape, core, 0, 1,
+                                     operand_shapes=[m.shape for m in (pre_a, pre_b, post) if m is not None])
+            if cut is not None:
+                kw = dict(pre_a=cut.cut(pre_a), pre_b=cut.cut(pre_b), post=cut.cut(post), device=self._host_device(da_a))
+                spec_b = (cut.axis(spec_b[0]),) + spec_b[1:]
+                if second.folded:
+                    _, seam, skip, mirror, period = _fold_plan(self, second.ax_name, dims, shape, 1)
+                    y = ops.stencil_pair_host_fold(cut.cut(fa.data), cut.cut(fb.data), spec_a, spec_b, cut.axis(seam),
+                                                   skip, mirror, period, sub, negate=negate, **kw)
                 else:
-                    y = ops.stencil_pair_host(cut(fa.data), cut(fb.data), spec_a, spec_b, sub, **kw)
+                    y = ops.stencil_pair_host(cut.cut(fa.data), cut.cut(fb.data), spec_a, spec_b, sub, **kw)
                 return finish(y.reshape(shape))
         xa, _ = as_device_tensor(fa.data, dev)
         xb, _ = as_device_tensor(fb.data, dev)
@@ -880,9 +833,9 @@ class Grid:
         pre_b = self._metric_tensor(self.get_metric(fb, mb_ax), fb.dims, xb) if mb_ax else None
         post = self._metric_tensor(self.get_metric(probe, divide_by), out_dims_a, xa) if divide_by else None
         halo = {}
-        if second["folded"]:
-            halo["halo_lo_b"], halo["halo_hi_b"] = fold_halo_planes(self, second["ax"], fb.dims, xb, second["lo"],
-                                                                    second["pad"], pre=pre_b, negate=negate)
+        if second.folded:
+            halo["halo_lo_b"], halo["halo_hi_b"] = fold_halo_planes(self, second.ax_name, fb.dims, xb, second.lo,
+                                                                    second.pad_mode, pre=pre_b, negate=negate)
         y = ops.stencil_pair(xa, xb, spec_a, spec_b, sub, pre_a=pre_a, pre_b=pre_b, post=post, **halo)
         return finish(result_like(y, host))
 
@@ -979,123 +932,156 @@ class Grid:
         paddings = self._complete_user_kwargs_using_axis_defaults(padding, "padding")
         fills = self._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
 
-        host_input = not da.is_device
-        # numpy-backed field, one axis: stream slabs through the GPU (xg_cumscan_host, or its _fold / _connected
-        # twin where the padded edge crosses a north fold or a face connection) instead of one un-overlapped
-        # upload + download around the kernel
-        host_stream = (host_input and len(axis) == 1
-                       and np.asarray(da.data).dtype in (np.float32, np.float64))
-        data = da
+        def plan(ax_name):
+            return self._cumsum_axis(da, ax_name, to, reverse, metric_weighted, paddings, fills)
 
-        def to_device(data):
-            x, _ = as_device_tensor(data.data, self._device_for(da))
-            return data._replace(data=x)
-
-        if not host_stream:
-            data = to_device(data)
+        if len(axis) == 1 and _is_host_float(da):
+            res = self._cumsum_host(da, plan(axis[0]), paddings, padding, fill_value, _pre_weight)
+            if res is not None:
+                return self._wrap_out(res, as_xarray)
+        x, _ = as_device_tensor(da.data, self._device_for(da))
+        data = da._replace(data=x)
         for ax_i, ax_name in enumerate(axis):
-            ax = self.axes[ax_name]
-            pos, dim = ax._get_position_name(da)
+            s = plan(ax_name)
             input_da = data
-            ax_reverse = bool(reverse.get(ax.name, False))
-            weighted = metric_weighted.get(ax.name) if isinstance(metric_weighted, dict) else None
-            ax_to = to.get(ax.name) if isinstance(to, dict) else None
-            if ax_to is None:
-                ax_to = ax._default_shifts[pos]
-            try:
-                trim, (pad_lo, pad_hi) = (_CUMSUM_REV if ax_reverse else _CUMSUM_FWD)[(pos, ax_to)]
-            except KeyError:
-                raise ValueError(
-                    f"From `{pos}` to `{ax_to}` is not a valid position "
-                    f"shift for cumsum operation along axis {ax}."
-                )
-            folded, ax_padding = fold_edges(self, ax.name, paddings[ax.name], pad_hi)
-            if (pad_lo or pad_hi) and ax_padding is None and self._face_connections is None:
-                raise ValueError(
-                    f"No boundary condition was specified for axis {ax.name!r}, but the "
-                    f"requested operation needs to pad it. Set a boundary condition, "
-                    f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                    f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                    f"grid method."
-                )
-            new_dim = ax.coords[ax_to]
-            out_dims = tuple(new_dim if d == dim else d for d in data.dims)
-            axis_num = data.get_axis_num(dim)
+            out_dims = tuple(s.new_dim if d == s.dim else d for d in data.dims)
+            axis_num = data.get_axis_num(s.dim)
             pre_t = post_t = None
             probe = DataArray.__new__(DataArray)
             probe._dims = out_dims
-            fv = fills[ax.name] if fills[ax.name] is not None else 0.0
-            bc = ax_padding if (pad_lo or pad_hi) else None
-            halo = None  # the fold or face connection a streamed call's padded edge crosses
-            if host_stream and (self._face_connections is not None or ax.name in self._folds):
-                if weighted and _pre_weight is not None:
-                    host_stream = False  # not streamed (below), but works on the whole-field route
-                elif self._face_connections is not None and (pad_lo or pad_hi):
-                    if paddings[ax.name] not in (None, "periodic", "fill", "extend"):
-                        host_stream = False  # e.g. a per-side mapping: pad() has the say
-                    elif ax.name in _get_all_connection_axes(self._face_connections, self._facedim):
-                        halo = "connected"
-                    else:  # e.g. Z on LLC: the basic boundary, checked as pad() checks it
-                        bc, fv = connected_edge_mode(self, ax.name, pad_lo, pad_hi, padding, fill_value,
-                                                     data.sizes[self._facedim])
-                elif folded:
-                    halo = "fold"
-                if not host_stream:
-                    data = to_device(data)
-            if host_stream:
-                fdt = np.asarray(data.data).dtype
-                if weighted:
-                    pre_t = self._metric_host(self.get_metric(data, weighted), data.dims, fdt)
-                    post_t = self._metric_host(self.get_metric(probe, weighted), out_dims, fdt)
-                if _pre_weight is not None:  # cumint: the metric product rides on the kernel's pre operand
-                    if pre_t is not None:
-                        raise NotImplementedError("cumint with metric_weighted on a host array: pass a device array")
-                    pre_t = self._metric_host(_pre_weight, data.dims, fdt)
-                if halo is not None:
-                    y = _cumsum_halo_host(self, halo, np.asarray(data.data), data.dims, ax.name, dim, ax_reverse,
-                                          trim, pad_lo, pad_hi, padding, fill_value, pre_t, post_t,
-                                          self._host_device(da))
-                    if y is None:  # a layout that does not stream
-                        host_stream = False
-                        pre_t = post_t = None
-                        data = to_device(data)
-            if not host_stream:
-                if weighted:
-                    pre_t = self._metric_tensor(self.get_metric(data, weighted), data.dims, data.data)
-                    post_t = self._metric_tensor(self.get_metric(probe, weighted), out_dims, data.data)
-                if _pre_weight is not None and ax_i == 0:
-                    w_t = self._metric_tensor(_pre_weight, data.dims, data.data)
-                    if pre_t is None:
-                        pre_t = w_t  # (da * w) is formed inside the scan kernel: 8 B/cell instead of 20
-                    else:  # two roundings in the reference, (da * w) * metric: keep them
-                        data = data._replace(data=ops.binary("mul", data.data, w_t))
-            if host_stream:
-                if halo is None:
-                    y = ops.cumscan_host(np.asarray(data.data), axis_num, ax_reverse, trim, pad_lo, pad_hi, bc, fv,
-                                         pre=pre_t, post=post_t, skipna=True, device=self._host_device(da))
-            elif (self._face_connections is not None and (pad_lo or pad_hi)) or folded:
+            if s.weighted:
+                pre_t = self._metric_tensor(self.get_metric(data, s.weighted), data.dims, data.data)
+                post_t = self._metric_tensor(self.get_metric(probe, s.weighted), out_dims, data.data)
+            if _pre_weight is not None and ax_i == 0:
+                w_t = self._metric_tensor(_pre_weight, data.dims, data.data)
+                if pre_t is None:
+                    pre_t = w_t  # (da * w) is formed inside the scan kernel: 8 B/cell instead of 20
+                else:  # two roundings in the reference, (da * w) * metric: keep them
+                    data = data._replace(data=ops.binary("mul", data.data, w_t))
+            if (self._face_connections is not None and (s.pad_lo or s.pad_hi)) or s.folded:
                 # the reference pads the cumsum'd data with ``pad`` (grid.py:1385-1391), which on a
                 # connected grid takes the halo from the neighbour face and across a north fold
                 # mirrors the scanned rows: scan + trim in the kernel, halo through ``pad``, metric
                 # divide last
-                y = ops.cumscan(data.data, axis_num, ax_reverse, trim, 0, 0, None, fv, pre=pre_t,
+                y = ops.cumscan(data.data, axis_num, s.reverse, s.trim, 0, 0, None, s.fill, pre=pre_t,
                                 post=None, skipna=True)
                 scanned = DataArray(y, dims=data.dims, name=da.name, attrs=da.attrs)
-                y = pad(scanned, grid=self, padding_width={ax.name: (pad_lo, pad_hi)}, padding=padding,
+                y = pad(scanned, grid=self, padding_width={ax_name: (s.pad_lo, s.pad_hi)}, padding=padding,
                         fill_value=fill_value).data
                 if post_t is not None:
                     y = ops.binary("div", y, post_t)
             else:
-                y = ops.cumscan(data.data, axis_num, ax_reverse, trim, pad_lo, pad_hi, bc, fv, pre=pre_t,
+                y = ops.cumscan(data.data, axis_num, s.reverse, s.trim, s.pad_lo, s.pad_hi, s.bc, s.fill, pre=pre_t,
                                 post=post_t, skipna=True)
             coordless = DataArray(y, dims=out_dims, name=da.name, attrs=da.attrs)
             data = _reattach_coords(
-                [coordless], grid=self, padding_width={ax.name: (pad_lo, pad_hi)},
-                out_core_dim_names={new_dim}, input_args=[input_da],
+                [coordless], grid=self, padding_width={ax_name: (s.pad_lo, s.pad_hi)},
+                out_core_dim_names={s.new_dim}, input_args=[input_da],
             )[0]
-        if host_input and not host_stream:
+        if not da.is_device:
             data = data._replace(data=result_like(data.data, True))
         return self._wrap_out(data, as_xarray)
+
+    def _cumsum_axis(self, da, ax_name, to, reverse, metric_weighted, paddings, fills) -> "_ScanAxis":
+        """The shift table entry, boundary and metric of one axis of ``cumsum``; raises for an invalid shift and
+        for a padded axis without a boundary condition."""
+        ax = self.axes[ax_name]
+        pos, dim = ax._get_position_name(da)
+        ax_reverse = bool(reverse.get(ax.name, False))
+        weighted = metric_weighted.get(ax.name) if isinstance(metric_weighted, dict) else None
+        ax_to = to.get(ax.name) if isinstance(to, dict) else None
+        if ax_to is None:
+            ax_to = ax._default_shifts[pos]
+        try:
+            trim, (pad_lo, pad_hi) = (_CUMSUM_REV if ax_reverse else _CUMSUM_FWD)[(pos, ax_to)]
+        except KeyError:
+            raise ValueError(
+                f"From `{pos}` to `{ax_to}` is not a valid position "
+                f"shift for cumsum operation along axis {ax}."
+            )
+        folded, ax_padding = fold_edges(self, ax.name, paddings[ax.name], pad_hi)
+        if (pad_lo or pad_hi) and ax_padding is None and self._face_connections is None:
+            raise missing_boundary_error(ax.name)
+        fv = fills[ax.name] if fills[ax.name] is not None else 0.0
+        return _ScanAxis(ax.name, dim, ax.coords[ax_to], ax_reverse, weighted, trim, pad_lo, pad_hi, folded,
+                         ax_padding if (pad_lo or pad_hi) else None, fv)
+
+    def _cumsum_host(self, da, s, paddings, padding, fill_value, pre_weight):
+        """One axis of ``cumsum`` on the numpy field ``da`` streamed through the GPU in slabs instead of one
+        un-overlapped upload + download around the kernel: ``xg_cumscan_host``, or ``xg_cumscan_host_fold`` /
+        ``_connected`` where the padded edge crosses a north fold or a face connection.  Those two run per slab
+        the device route's scan, halo of the scanned field (as ``pad`` builds it) and divide by the post metric;
+        their slabs are cut as the stencils cut them (``grid_ufunc._host_stream_route``) and the halo is planned
+        for the scanned, merged layout.  Returns the result, or None: the whole-field route (a fold or connected
+        call with both cumint and metric_weighted, a per-side padding mapping, no batch dim in front of the halo
+        dims, a fold the plan cannot mirror)."""
+        from . import ops
+        from .padding import _axis_dim, _fold_plan, connected_halo_program
+
+        bc, fv, halo = s.bc, s.fill, None  # halo: the fold or face connection the padded edge crosses
+        if self._face_connections is not None or s.ax_name in self._folds:
+            if s.weighted and pre_weight is not None:
+                return None
+            if self._face_connections is not None and (s.pad_lo or s.pad_hi):
+                if paddings[s.ax_name] not in (None, "periodic", "fill", "extend"):
+                    return None  # e.g. a per-side mapping: pad() has the say
+                if s.ax_name in _get_all_connection_axes(self._face_connections, self._facedim):
+                    halo = "connected"
+                else:  # e.g. Z on LLC: the basic boundary, checked as pad() checks it
+                    bc, fv = connected_edge_mode(self, s.ax_name, s.pad_lo, s.pad_hi, padding, fill_value,
+                                                 da.sizes[self._facedim])
+            elif s.folded:
+                halo = "fold"
+        x, dims, shape = da.data, tuple(da.dims), [int(v) for v in da.shape]
+        out_dims = tuple(s.new_dim if d == s.dim else d for d in dims)
+        axis_num = dims.index(s.dim)
+        pre = post = None
+        if s.weighted:
+            probe = DataArray.__new__(DataArray)
+            probe._dims = out_dims
+            pre = self._metric_host(self.get_metric(da, s.weighted), dims, x.dtype)
+            post = self._metric_host(self.get_metric(probe, s.weighted), out_dims, x.dtype)
+        if pre_weight is not None:  # cumint: the metric product rides on the kernel's pre operand
+            if pre is not None:
+                raise NotImplementedError("cumint with metric_weighted on a host array: pass a device array")
+            pre = self._metric_host(pre_weight, dims, x.dtype)
+        device = self._host_device(da)
+        if halo is None:
+            y = ops.cumscan_host(x, axis_num, s.reverse, s.trim, s.pad_lo, s.pad_hi, bc, fv, pre=pre, post=post,
+                                 skipna=True, device=device)
+        else:
+            if halo == "fold":
+                core = [s.dim, _axis_dim(self, dims, self._folds[s.ax_name]["seam_axis"])]
+            else:
+                core = [s.dim, self._facedim] + [d for a in _get_all_connection_axes(self._face_connections,
+                                                                                       self._facedim)
+                                                 for d in self.axes[a].coords.values() if d in dims]
+            cut = _host_stream_route(halo, dims, shape, core, s.pad_lo, s.pad_hi,
+                                     operand_shapes=[m.shape for m in (pre, post) if m is not None])
+            if cut is None:
+                return None
+            scanned = list(shape)
+            scanned[axis_num] -= 0 if s.trim == "none" else 1
+            m_dims, m_scanned = cut.dims(dims), cut.shape(scanned)
+            kw = dict(pre=cut.cut(pre), post=cut.cut(post), skipna=True, device=device)
+            if halo == "fold":
+                try:
+                    _, seam, skip, mirror, period = _fold_plan(self, s.ax_name, m_dims, m_scanned, 1)
+                except NotImplementedError:
+                    return None
+                y = ops.cumscan_host_fold(cut.cut(x), cut.axis(axis_num), s.reverse, s.trim, seam, skip, mirror,
+                                          period, **kw)
+            else:
+                mode, fv = connected_edge_mode(self, s.ax_name, s.pad_lo, s.pad_hi, padding, fill_value,
+                                               shape[dims.index(self._facedim)])
+                program = connected_halo_program(self, s.ax_name, s.pad_lo, s.pad_hi, m_dims, m_scanned, mode)
+                y = ops.cumscan_host_connected(cut.cut(x), cut.axis(axis_num), s.reverse, s.trim, s.pad_lo,
+                                               s.pad_hi, fv, program, **kw)
+            scanned[axis_num] += s.pad_lo + s.pad_hi
+            y = y.reshape(scanned)
+        coordless = DataArray(y, dims=out_dims, name=da.name, attrs=da.attrs)
+        return _reattach_coords([coordless], grid=self, padding_width={s.ax_name: (s.pad_lo, s.pad_hi)},
+                                out_core_dim_names={s.new_dim}, input_args=[da])[0]
 
     def cumint(self, da, axis, **kwargs):
         """Cumulative integral: ``cumsum(da * get_metric(da, axis), axis)`` (grid.py:1607-1660)."""
@@ -1123,33 +1109,15 @@ class Grid:
             skipna = True  # xarray default for float data
         weight = self.get_metric(da, axis)
         dims = self._get_dims_from_axis(da, axis)
-        host_input = not da.is_device
-        if (host_input and len(dims) == 1 and np.asarray(da.data).dtype in (np.float32, np.float64)):
-            # numpy-backed field, one axis: slabs stream through the GPU (xg_wreduce_host)
-            arr = np.asarray(da.data)
-            axn = da.get_axis_num(dims[0])
-            w_np = self._metric_host(weight, da.dims, arr.dtype)
-            y = ops.wreduce_host(arr, axn, w_np, mode, bool(skipna), device=self._host_device(da))
-            res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ != dims[0]), name=da.name)
-            coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
-            return self._wrap_out(res.assign_coords(coords), as_xarray)
-        dev = self._device_for(da)
-        if (host_input and len(set(dims)) == len(dims) > 1 and dev.type == "cuda"
-                and np.asarray(da.data).dtype in (np.float32, np.float64)):
-            # numpy-backed field, several axes: the launches below run per slab (xg_wreduce_host_multi), with a
-            # weight that spans the slab dim streamed beside the field
-            arr = np.asarray(da.data)
-            w_np = self._metric_host(weight, da.dims, arr.dtype)
-            try:
-                y = ops.wreduce_host_multi(arr, [da.get_axis_num(d) for d in dims], w_np, mode, bool(skipna),
-                                           device=self._host_device(da))
-            except NotImplementedError:
-                y = None  # an empty reduced dim, or a single line: the whole field on the device
-            if y is not None:
-                res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ not in dims), name=da.name)
-                coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
-                return self._wrap_out(res.assign_coords(coords), as_xarray)
-        x, _ = as_device_tensor(da.data, dev)
+
+        def with_coords(res):
+            return res.assign_coords({k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)})
+
+        y = self._weighted_reduce_host(da, dims, weight, mode, skipna) if _is_host_float(da) else None
+        if y is not None:
+            res = DataArray(y, dims=tuple(x_ for x_ in da.dims if x_ not in dims), name=da.name)
+            return self._wrap_out(with_coords(res), as_xarray)
+        x, _ = as_device_tensor(da.data, self._device_for(da))
         cur = da._replace(data=x)
         wt = self._metric_tensor(weight, cur.dims, x)
         # several axes: the first pass (innermost listed dim) applies the weights, the others are plain sums
@@ -1179,11 +1147,30 @@ class Grid:
                 first = False
                 cur = DataArray(y, dims=tuple(x_ for x_ in cur.dims if x_ != d), name=da.name)
             res = cur
-        coords = {k: c for k, c in da.coords.items() if all(d in res.dims for d in c.dims)}
-        res = res.assign_coords(coords)
-        if host_input:
+        res = with_coords(res)
+        if not da.is_device:
             res = res._replace(data=result_like(res.data, True))
         return self._wrap_out(res, as_xarray)
+
+    def _weighted_reduce_host(self, da, dims, weight, mode, skipna):
+        """``integrate`` / ``average`` of the numpy field ``da`` over ``dims`` streamed through the GPU in slabs:
+        ``xg_wreduce_host`` for one dim, ``xg_wreduce_host_multi`` for several (the launches of the device route
+        run per slab, with a weight that spans the slab dim streamed beside the field).  Returns the reduced
+        array, or None: the whole-field route."""
+        from . import ops
+
+        if len(dims) == 1:
+            w_np = self._metric_host(weight, da.dims, da.data.dtype)
+            return ops.wreduce_host(da.data, da.get_axis_num(dims[0]), w_np, mode, bool(skipna),
+                                    device=self._host_device(da))
+        if not (len(set(dims)) == len(dims) > 1 and self._device_for(da).type == "cuda"):
+            return None
+        w_np = self._metric_host(weight, da.dims, da.data.dtype)
+        try:
+            return ops.wreduce_host_multi(da.data, [da.get_axis_num(d) for d in dims], w_np, mode, bool(skipna),
+                                          device=self._host_device(da))
+        except NotImplementedError:
+            return None  # an empty reduced dim, or a single line: the whole field on the device
 
     def integrate(self, da, axis, **kwargs):
         """Finite-volume integral ``(da * metric).sum(dim)`` (grid.py:1580-1605), fused."""
@@ -1251,56 +1238,58 @@ class Grid:
         return self._apply_vector_function(self.interp, vector, **kwargs)
 
 
+class _StencilTerm(NamedTuple):
+    """One built-in stencil (diff / interp / min / max) of a field along one axis, as the fused launches take it."""
+
+    op: str
+    ax_name: str
+    lo: int
+    hi: int
+    in_dim: str
+    out_dim: str
+    axis_num: int
+    pad_mode: Optional[str]
+    fill: float
+    folded: bool
+
+
+def _stencil_term(grid, funcname, da, ax_name, to, paddings, fills) -> _StencilTerm:
+    """Resolve ``funcname`` of ``da`` along ``ax_name`` to position ``to`` (None: the axis default shift): the
+    gridops ufunc and its padding, the dims in and out, the boundary (``paddings`` / ``fills`` completed with
+    the Axis defaults) and whether the north edge folds.  Raises for a position the axis does not have and for
+    a padded axis without a boundary condition."""
+    sig = grid._create_1d_grid_ufunc_signatures(da, axis=[ax_name], to={ax_name: to})[0]
+    grid_ufunc, _ = _select_grid_ufunc(funcname, sig, module=gridops)
+    dummy = grid_ufunc.signature.in_ax_names[0][0]  # the ufunc's own dummy axis name ("X")
+    lo, hi = (grid_ufunc.padding_width or {}).get(dummy, (0, 0))
+    from_pos, to_pos = sig.in_ax_positions[0][0], sig.out_ax_positions[0][0]
+    coords = grid.axes[ax_name].coords
+    if to_pos not in coords:
+        raise ValueError(f"Axis position ({ax_name}:{to_pos}) does not exist in grid")
+    folded, pad_mode, fill = _stencil_boundary(grid, ax_name, lo, hi, paddings, fills)
+    in_dim = coords[from_pos]
+    return _StencilTerm(funcname, ax_name, lo, hi, in_dim, coords[to_pos], da.get_axis_num(in_dim), pad_mode, fill,
+                        folded)
+
+
+class _ScanAxis(NamedTuple):
+    """One axis of ``Grid.cumsum``: its dims, direction, metric, shift table entry and boundary."""
+
+    ax_name: str
+    dim: str
+    new_dim: str
+    reverse: bool
+    weighted: Any
+    trim: str
+    pad_lo: int
+    pad_hi: int
+    folded: bool
+    bc: Optional[str]
+    fill: float
+
+
 # (from, to) -> (trim, (pad_lo, pad_hi)); transcription of the enumerated shifts of
 # reference grid.py:1326-1383
-def _cumsum_halo_host(grid, kind, x, dims, ax_name, dim, reverse, trim, pad_lo, pad_hi, padding, fill_value, pre,
-                      post, device):
-    """One axis of ``Grid.cumsum`` on the numpy field ``x`` whose padded edge crosses a north fold (``kind``
-    "fold") or a face connection ("connected"), streamed in slabs by ``xg_cumscan_host_fold`` /
-    ``_connected``: per slab the device route's scan, halo of the scanned field (as ``pad`` builds it) and
-    divide by ``post``.  The slabs are cut as the stencils cut them (``grid_ufunc._host_stream_route``); the
-    halo is planned for the scanned, merged layout.  Returns the result, or None when the layout does not stream
-    (no batch dim in front, or a fold the plan cannot mirror): the whole-field route then runs."""
-    from . import ops
-    from .grid_ufunc import _host_stream_route, _merge_leading
-    from .padding import _axis_dim, _fold_plan, connected_halo_program
-
-    dims = tuple(dims)
-    shape = [int(v) for v in x.shape]
-    axis_num = dims.index(dim)
-    if kind == "fold":
-        core = [dim, _axis_dim(grid, dims, grid._folds[ax_name]["seam_axis"])]
-    else:
-        core = [dim, grid._facedim] + [d for a in _get_all_connection_axes(grid._face_connections, grid._facedim)
-                                       for d in grid.axes[a].coords.values() if d in dims]
-    route = _host_stream_route(kind, dims, shape, core, pad_lo, pad_hi,
-                               operand_shapes=[m.shape for m in (pre, post) if m is not None])
-    if route is None:
-        return None
-    _, ndrop, nmerge = route
-    lead = ndrop + nmerge
-    cut = lambda a: None if a is None else _merge_leading(a, ndrop, nmerge)  # noqa: E731
-    m_dims = dims[ndrop:ndrop + 1] + dims[lead:]  # the merged batch dim keeps the name of its first dim
-    scanned = list(shape)
-    scanned[axis_num] -= 0 if trim == "none" else 1
-    m_scanned = [int(np.prod(scanned[ndrop:lead]))] + scanned[lead:]
-    ax = axis_num - lead + 1
-    kw = dict(pre=cut(pre), post=cut(post), skipna=True, device=device)
-    if kind == "fold":
-        try:
-            _, seam, skip, mirror, period = _fold_plan(grid, ax_name, m_dims, m_scanned, 1)
-        except NotImplementedError:
-            return None
-        out = ops.cumscan_host_fold(cut(x), ax, reverse, trim, seam, skip, mirror, period, **kw)
-    else:
-        mode, fv = connected_edge_mode(grid, ax_name, pad_lo, pad_hi, padding, fill_value,
-                                       shape[dims.index(grid._facedim)])
-        program = connected_halo_program(grid, ax_name, pad_lo, pad_hi, m_dims, m_scanned, mode)
-        out = ops.cumscan_host_connected(cut(x), ax, reverse, trim, pad_lo, pad_hi, fv, program, **kw)
-    scanned[axis_num] += pad_lo + pad_hi
-    return out.reshape(scanned)
-
-
 _CUMSUM_FWD = {
     ("center", "right"): ("none", (0, 0)),
     ("left", "center"): ("none", (0, 0)),

@@ -21,12 +21,12 @@ from __future__ import annotations
 import re
 import string
 import collections.abc
-from typing import Any, Callable, Dict, List, Mapping, Optional, Sequence, Tuple, Union, get_type_hints
+from typing import Any, Callable, Dict, List, Mapping, NamedTuple, Optional, Sequence, Tuple, Union, get_type_hints
 
 import numpy as np
 
 from .labeled import DataArray
-from .padding import pad
+from .padding import fold_edges, missing_boundary_error, pad
 
 _AXIS_NAME = r"\w+"
 _AXIS_POSITION = "(?:center|left|right|inner|outer)"
@@ -603,27 +603,18 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             op, da, da if raw_arg is None else raw_arg, other_component, grid, ax_name, in_dim,
             out_dim, padding_width_real, padding, fill_value, pre_metric, post_metric_fn,
         )
-    from .padding import fold_edges, fold_halo_planes
+    from .padding import fold_halo_planes
 
     lo, hi = padding_width_real.get(ax_name, (0, 0))
     paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
     fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
-    folded, ax_padding = fold_edges(grid, ax_name, paddings[ax_name], hi)
-    if (lo or hi) and ax_padding is None:
-        raise ValueError(
-            f"No boundary condition was specified for axis {ax_name!r}, but the "
-            f"requested operation needs to pad it. Set a boundary condition, "
-            f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-            f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-            f"grid method."
-        )
+    folded, ax_padding, fv = _stencil_boundary(grid, ax_name, lo, hi, paddings, fills)
     axis_num = da.get_axis_num(in_dim)
     out_dims = tuple(out_dim if d == in_dim else d for d in da.dims)
     out_shape = list(da.shape)
     out_shape[axis_num] = da.shape[axis_num] + lo + hi - 1
     post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
     bc = ax_padding if (lo or hi) else None
-    fv = fills[ax_name] if fills[ax_name] is not None else 0.0
 
     if _is_host_float(da) and (not folded or grid._device_for(da).type == "cuda"):
         # host field: stream slabs H2D -> kernel -> D2H inside the library (xg_stencil2_host, or
@@ -636,22 +627,18 @@ def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_r
             from .padding import _axis_dim, _fold_plan
 
             core.append(_axis_dim(grid, dims, grid._folds[ax_name]["seam_axis"]))
-        route = _host_stream_route("fold" if folded else "plain", dims, shape, core, lo, hi,
-                                   operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
-        if route is not None:
-            _, ndrop, nmerge = route
-            cut = lambda a: _merge_leading(a, ndrop, nmerge)  # noqa: E731
-            x = cut(da.data)
-            ax = axis_num - ndrop - nmerge + 1
-            kw = dict(pre=None if pre_h is None else cut(pre_h), post=None if post_h is None else cut(post_h),
-                      device=grid._host_device(da))
+        cut = _host_stream_route("fold" if folded else "plain", dims, shape, core, lo, hi,
+                                 operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
+        if cut is not None:
+            kw = dict(pre=cut.cut(pre_h), post=cut.cut(post_h), device=grid._host_device(da))
             try:
                 if folded:
                     _, seam, skip, mirror, period = _fold_plan(grid, ax_name, dims, shape, 1)
-                    out = ops.stencil2_host_fold(x, ax, op, lo, hi, bc, fv, seam - ndrop - nmerge + 1, skip, mirror,
-                                                 period, negate=isinstance(raw_arg, dict), **kw)
+                    out = ops.stencil2_host_fold(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, bc, fv,
+                                                 cut.axis(seam), skip, mirror, period,
+                                                 negate=isinstance(raw_arg, dict), **kw)
                 else:
-                    out = ops.stencil2_host(x, ax, op, lo, hi, bc, fv, **kw)
+                    out = ops.stencil2_host(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, bc, fv, **kw)
                 return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
             except NotImplementedError:
                 pass  # e.g. periodic halo + pre-metric along the outermost axis: whole-field path below
@@ -672,6 +659,43 @@ def _is_host_float(da) -> bool:
     return not da.is_device and isinstance(da.data, np.ndarray) and da.data.dtype in (np.float32, np.float64)
 
 
+def _stencil_boundary(grid, ax_name, lo, hi, paddings, fills):
+    """``(north folds, boundary mode, fill value)`` of a stencil that pads ``ax_name`` by ``lo, hi``, from the
+    per-axis ``paddings`` / ``fills`` (per call, else the Axis defaults).  Raises when the stencil pads an axis
+    that has no boundary condition."""
+    folded, pad_mode = fold_edges(grid, ax_name, paddings[ax_name], hi)
+    if (lo or hi) and pad_mode is None:
+        raise missing_boundary_error(ax_name)
+    return folded, pad_mode, (fills[ax_name] if fills[ax_name] is not None else 0.0)
+
+
+class HostCut(NamedTuple):
+    """How a numpy field is cut into slabs along dim 0 (``_host_stream_route``): its first ``ndrop`` dims (of
+    extent 1) are dropped and the next ``nmerge`` merged into one dim 0, the slab dim."""
+
+    kind: str
+    ndrop: int
+    nmerge: int
+
+    def cut(self, a):
+        """``a`` (the field, or a metric with 1 where it broadcasts) in the merged layout; None stays None."""
+        return None if a is None else _merge_leading(a, self.ndrop, self.nmerge)
+
+    def axis(self, i):
+        """Dim ``i`` of the field (one behind the merged dims) in the merged layout."""
+        return i - self.ndrop - self.nmerge + 1
+
+    def dims(self, dims):
+        """The merged dim names: the merged batch dim keeps the name of its first dim."""
+        dims = tuple(dims)
+        return dims[self.ndrop:self.ndrop + 1] + dims[self.ndrop + self.nmerge:]
+
+    def shape(self, shape):
+        """The merged shape."""
+        lead = self.ndrop + self.nmerge
+        return [int(np.prod(shape[self.ndrop:lead]))] + [int(v) for v in shape[lead:]]
+
+
 def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_ok=True, operand_shapes=()):
     """Whether a numpy field streams through a host slab pipeline, and how it is cut.
 
@@ -681,15 +705,15 @@ def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_
     axes).  The slabs are cut along dim 0: leading size-1 dims are dropped first, then the leading batch dims
     (those before the first core dim) are merged into one dim 0 -- as far as every broadcast operand (metric
     ``operand_shapes``, 1 where it broadcasts) merges with them.  A plain grid cuts the field's own dim 0 (no
-    merge), which may be the operated dim.  Returns ``(kind, dims dropped, dims merged)``, or None for the
-    whole-field device path: a fold, connected or pair field with no batch dim in front, a halo wider than
-    one cell, a pre-metric or a partner component that cannot stream beside the field on a connected grid."""
+    merge), which may be the operated dim.  Returns the :class:`HostCut`, or None for the whole-field device
+    path: a fold, connected or pair field with no batch dim in front, a halo wider than one cell, a pre-metric
+    or a partner component that cannot stream beside the field on a connected grid."""
     first = min(list(dims).index(d) for d in core_dims)
     ndrop = 0
     while ndrop < first and shape[ndrop] == 1:
         ndrop += 1
     if kind == "plain":
-        return kind, ndrop, 1
+        return HostCut(kind, ndrop, 1)
     if lo > 1 or hi > 1 or first == ndrop or (kind == "connected" and (pre or not partner_ok)):
         return None
     nmerge = first - ndrop
@@ -700,7 +724,7 @@ def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_
 
     while nmerge > 1 and not all(merges(m, nmerge) for m in operand_shapes):
         nmerge -= 1
-    return kind, ndrop, nmerge
+    return HostCut(kind, ndrop, nmerge)
 
 
 def _merge_leading(a, ndrop, nmerge):
@@ -737,24 +761,19 @@ def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_di
     partner_ok = not isvector or (
         not partner.is_device and isinstance(partner.data, np.ndarray) and len(partner.dims) == len(dims)
         and tuple(partner.dims[:first]) == dims[:first] and tuple(partner.shape[:first]) == tuple(shape[:first]))
-    route = _host_stream_route("connected", dims, shape, core, lo, hi, partner_ok=partner_ok,
-                               operand_shapes=[post_h.shape] if post_h is not None else [])
-    if route is None:
+    cut = _host_stream_route("connected", dims, shape, core, lo, hi, partner_ok=partner_ok,
+                             operand_shapes=[post_h.shape] if post_h is not None else [])
+    if cut is None:
         return None
-    _, ndrop, nmerge = route
-    cut = lambda a: _merge_leading(a, ndrop, nmerge)  # noqa: E731
-    lead = ndrop + nmerge
-    m_dims = dims[ndrop:ndrop + 1] + dims[lead:]  # the merged batch dim keeps the name of its first dim
-    x = cut(da.data)
+    m_dims = cut.dims(dims)
     q = partner_layout = None
     if isvector:
-        q = cut(partner.data)
-        partner_layout = (tuple(partner.dims[ndrop:ndrop + 1] + partner.dims[lead:]), tuple(q.shape))
-    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, list(x.shape), mode, vectoraxis,
+        q = cut.cut(partner.data)
+        partner_layout = (cut.dims(partner.dims), tuple(q.shape))
+    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, cut.shape(shape), mode, vectoraxis,
                                      partner_layout)
-    out = ops.stencil2_host_connected(x, m_dims.index(in_dim), op, lo, hi, fv, program, partner=q,
-                                      post=None if post_h is None else cut(post_h),
-                                      device=grid._host_device(da))
+    out = ops.stencil2_host_connected(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program, partner=q,
+                                      post=cut.cut(post_h), device=grid._host_device(da))
     return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
 
 

@@ -49,6 +49,45 @@ def _norm_axis(axis: int, ndim: int) -> int:
     return axis % ndim
 
 
+def _check_padding(padding) -> None:
+    if padding not in _capi.BCS:
+        raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}")
+
+
+def _stencil_specs(specs, ndim: int, fused: bool):
+    """C-ABI values of stencil ``specs`` ``[(axis, op, lo, hi, padding, fill), ...]``: lists of axes, op codes, lo,
+    hi, boundary codes and fills.  ``fused`` (one multi-axis launch): the boundary of a padded axis is periodic,
+    fill or extend (NotImplementedError for another, ValueError for none) and each axis appears once."""
+    axes, opc, los, his, bcs, fills = [], [], [], [], [], []
+    for axis, op, lo, hi, padding, fill in specs:
+        axes.append(_norm_axis(axis, ndim))
+        if op not in _capi.OPS:
+            raise ValueError(f"unknown op {op!r}")
+        if fused and padding not in ("periodic", "fill", "extend", None):
+            raise NotImplementedError(f"fused multi-axis stencils support periodic / fill / extend, not {padding!r}")
+        if fused and (lo or hi) and padding is None:
+            raise ValueError("no boundary condition was specified but the operation needs to pad the axis")
+        _check_padding(padding)
+        opc.append(_capi.OPS[op])
+        los.append(int(lo))
+        his.append(int(hi))
+        bcs.append(_capi.BCS[padding] if (lo or hi) else 0)
+        fills.append(float(0.0 if fill is None else fill))
+    if fused and len(set(axes)) != len(axes):
+        raise ValueError("each axis may appear only once")
+    return axes, opc, los, his, bcs, fills
+
+
+def _bins_order(diffs) -> int:
+    """``flip`` of monotonic target bins with steps ``diffs``: 1 when they decrease, 0 when they increase
+    (transform.py:167-176)."""
+    if bool((diffs < 0).all()):
+        return 1
+    if bool((diffs > 0).all()):
+        return 0
+    raise ValueError("Target values are not monotonic")
+
+
 def _operand(m: Optional[torch.Tensor], shape: Sequence[int], like: torch.Tensor, what: str):
     """Return (keepalive tensor, data_ptr, int64[ndim] strides) for a broadcast operand."""
     if m is None:
@@ -92,10 +131,7 @@ def stencil2(
     _require_cuda(x, "field")
     if op not in _capi.OPS:
         raise ValueError(f"unknown op {op!r}")
-    if padding not in _capi.BCS:
-        raise ValueError(
-            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}"
-        )
+    _check_padding(padding)
     x = x.contiguous()
     axis = _norm_axis(axis, x.dim())
     shape = list(x.shape)
@@ -147,25 +183,8 @@ def stencil_multi(x: torch.Tensor, specs: Sequence[Tuple[int, str, int, int, Opt
         raise ValueError("stencil_multi fuses 2 or 3 axes")
     x = x.contiguous()
     shape = list(x.shape)
-    out_shape = list(shape)
-    axes, opc, los, his, bcs, fills = [], [], [], [], [], []
-    for axis, op, lo, hi, padding, fill in specs:
-        axis = _norm_axis(axis, x.dim())
-        if op not in _capi.OPS:
-            raise ValueError(f"unknown op {op!r}")
-        if padding not in ("periodic", "fill", "extend", None):
-            raise NotImplementedError(f"fused multi-axis stencils support periodic / fill / extend, not {padding!r}")
-        if (lo or hi) and padding is None:
-            raise ValueError("no boundary condition was specified but the operation needs to pad the axis")
-        axes.append(axis)
-        opc.append(_capi.OPS[op])
-        los.append(int(lo))
-        his.append(int(hi))
-        bcs.append(_capi.BCS[padding] if (lo or hi) else 0)
-        fills.append(float(fill))
-        out_shape[axis] = shape[axis] + lo + hi - 1
-    if len(set(axes)) != len(axes):
-        raise ValueError("each axis may appear only once")
+    axes, opc, los, his, bcs, fills = _stencil_specs(specs, x.dim(), fused=True)
+    out_shape = _multi_out_shape(shape, axes, los, his)
     if len(set(opc)) != 1:
         # mixed operators: not a Grid-level case; same result through the per-axis kernel
         out = x
@@ -186,15 +205,19 @@ def stencil_multi(x: torch.Tensor, specs: Sequence[Tuple[int, str, int, int, Opt
     return out
 
 
+def _multi_out_shape(shape, axes, los, his):
+    out_shape = list(shape)
+    for axis, lo, hi in zip(axes, los, his):
+        out_shape[axis] = shape[axis] + lo + hi - 1
+    return out_shape
+
+
 def pad(x: torch.Tensor, axis: int, lo: int, hi: int, padding: Optional[str],
         fill_value: float = 0.0) -> torch.Tensor:
     """The padded array itself (padding.py:575-616), one axis."""
     lib = _capi.load()
     _require_cuda(x, "field")
-    if padding not in _capi.BCS:
-        raise ValueError(
-            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}"
-        )
+    _check_padding(padding)
     x = x.contiguous()
     axis = _norm_axis(axis, x.dim())
     shape = list(x.shape)
@@ -381,10 +404,7 @@ def cumscan(
     """Cumulative sum with xgcm's trim / pad table fused (grid.py:1306-1414)."""
     lib = _capi.load()
     _require_cuda(x, "field")
-    if padding not in _capi.BCS:
-        raise ValueError(
-            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}"
-        )
+    _check_padding(padding)
     x = x.contiguous()
     axis = _norm_axis(axis, x.dim())
     shape = list(x.shape)
@@ -498,13 +518,8 @@ def vinterp_conservative(phi: torch.Tensor, theta: torch.Tensor, target_bins: to
         raise ValueError(
             f"theta needs {tshape[axis]} cell bounds along the axis, got {theta.shape[axis]}"
         )  # transform.py:162 assert phi.shape[-1] == theta.shape[-1] - 1
-    diffs = target_bins[1:] - target_bins[:-1]
-    if bool((diffs < 0).all()):  # transform.py:167-176
-        flip, bins = 1, torch.flip(target_bins, dims=(0,)).contiguous()
-    elif bool((diffs > 0).all()):
-        flip, bins = 0, target_bins.contiguous()
-    else:
-        raise ValueError("Target values are not monotonic")
+    flip = _bins_order(target_bins[1:] - target_bins[:-1])
+    bins = (torch.flip(target_bins, dims=(0,)) if flip else target_bins).contiguous()
     keep, th_ptr, th_st = _operand(theta, tshape, phi, "theta")
     m = int(bins.numel())
     out_shape = [s for d, s in enumerate(shape) if d != axis] + [m - 1]
@@ -556,6 +571,29 @@ def _host_operand(m: Optional[np.ndarray], shape: Sequence[int], dtype, what: st
     return m, m.ctypes.data, _capi.i64_array(strides)
 
 
+def _host_field(x, what, cast=True):
+    """``x`` C-contiguous for a host twin (with ``cast``, a non-float field as float64), on a machine with a CUDA
+    device."""
+    if not isinstance(x, np.ndarray):
+        raise TypeError(f"{what} must be a numpy array")
+    if not torch.cuda.is_available():
+        raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
+    if cast and x.dtype not in (np.float32, np.float64):
+        x = x.astype(np.float64)
+    if not x.flags.c_contiguous:
+        x = np.ascontiguousarray(x)
+    return x
+
+
+def _host_out(out, shape, dtype):
+    """The page-locked result of a host twin, or the caller's ``out`` after checking it."""
+    if out is None:
+        return pinned_empty(shape, dtype)
+    if list(out.shape) != list(shape) or out.dtype != dtype or not out.flags.c_contiguous:
+        raise ValueError("out has wrong shape/dtype/layout")
+    return out
+
+
 def pinned_empty(shape, dtype=np.float32) -> np.ndarray:
     """A page-locked numpy array (torch's caching host allocator owns the memory)."""
     tdt = {np.dtype("float32"): torch.float32, np.dtype("float64"): torch.float64}[np.dtype(dtype)]
@@ -593,26 +631,15 @@ def stencil2_host(
 def _host_stencil_prep(x, axis, op, lo, hi, padding, pre, post, out, device, what):
     """Checks and buffers shared by the host stencil twins: (contiguous x, shape, axis, out, pre operand,
     post operand, device index)."""
-    if not isinstance(x, np.ndarray):
-        raise TypeError(f"{what} takes numpy arrays")
-    if not torch.cuda.is_available():
-        raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
+    x = _host_field(x, f"{what}: field", cast=False)
     if op not in _capi.OPS:
         raise ValueError(f"unknown op {op!r}")
-    if padding not in _capi.BCS:
-        raise ValueError(
-            f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}"
-        )
-    if not x.flags.c_contiguous:
-        x = np.ascontiguousarray(x)
+    _check_padding(padding)
     axis = _norm_axis(axis, x.ndim)
     shape = list(x.shape)
     out_shape = list(shape)
     out_shape[axis] = shape[axis] + lo + hi - 1
-    if out is None:
-        out = pinned_empty(out_shape, x.dtype)
-    elif list(out.shape) != out_shape or out.dtype != x.dtype or not out.flags.c_contiguous:
-        raise ValueError("out has wrong shape/dtype/layout")
+    out = _host_out(out, out_shape, x.dtype)
     pre_op = _host_operand(pre, shape, x.dtype, "pre metric")
     post_op = _host_operand(post, out_shape, x.dtype, "post metric")
     dev = host_device_arg(device)
@@ -748,20 +775,12 @@ def stencil_pair(a: torch.Tensor, b: torch.Tensor, spec_a, spec_b, subtract: int
 def _host_pair_prep(a, b, spec_a, spec_b, pre_a, pre_b, post, out, device, what):
     """Checks and buffers shared by the host pair twins: (a, b, shape, C-ABI term values, the three operands,
     out, device index)."""
-    for x in (a, b):
-        if not isinstance(x, np.ndarray):
-            raise TypeError(f"{what} takes numpy arrays")
-    if not torch.cuda.is_available():
-        raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
+    a, b = _host_field(a, f"{what}: field a", cast=False), _host_field(b, f"{what}: field b", cast=False)
     if a.shape != b.shape or a.dtype != b.dtype:
         raise ValueError(f"{what}: both fields must have the same shape and dtype")
-    a, b = np.ascontiguousarray(a), np.ascontiguousarray(b)
     term_a, term_b = _pair_specs(spec_a, spec_b, a.ndim)
     shape = list(a.shape)
-    if out is None:
-        out = pinned_empty(shape, a.dtype)
-    elif list(out.shape) != shape or out.dtype != a.dtype or not out.flags.c_contiguous:
-        raise ValueError("out has wrong shape/dtype/layout")
+    out = _host_out(out, shape, a.dtype)
     ops_ = [_host_operand(m, shape, a.dtype, w) for m, w in ((pre_a, "pre metric a"), (pre_b, "pre metric b"),
                                                              (post, "post metric"))]
     dev = host_device_arg(device)
@@ -804,16 +823,6 @@ def stencil_pair_host_fold(a: np.ndarray, b: np.ndarray, spec_a, spec_b, seam_ax
 
 
 # --------------------------------------------------------------------------- host twins (slab pipelines)
-def _host_field(x, what):
-    if not isinstance(x, np.ndarray):
-        raise TypeError(f"{what} must be a numpy array")
-    if not torch.cuda.is_available():
-        raise RuntimeError("xgcm_b200 needs a CUDA device: the stencil engine has no CPU fallback")
-    if x.dtype not in (np.float32, np.float64):
-        x = x.astype(np.float64)
-    if not x.flags.c_contiguous:
-        x = np.ascontiguousarray(x)
-    return x
 
 
 def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: HostDevice = None):
@@ -826,22 +835,8 @@ def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: HostDevice = No
     x = _host_field(x, "field")
     k = len(specs)
     shape = list(x.shape)
-    axes, ops_, los, his, bcs, fills, out_shapes = [], [], [], [], [], [], []
-    for axis, op, lo, hi, padding, fill in specs:
-        if op not in _capi.OPS:
-            raise ValueError(f"unknown op {op!r}")
-        if padding not in _capi.BCS:
-            raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}")
-        axis = _norm_axis(axis, x.ndim)
-        axes.append(axis)
-        ops_.append(_capi.OPS[op])
-        los.append(int(lo))
-        his.append(int(hi))
-        bcs.append(_capi.BCS[padding] if (lo or hi) else 0)
-        fills.append(float(0.0 if fill is None else fill))
-        osh = list(shape)
-        osh[axis] = shape[axis] + lo + hi - 1
-        out_shapes.append(osh)
+    axes, ops_, los, his, bcs, fills = _stencil_specs(specs, x.ndim, fused=False)
+    out_shapes = [_multi_out_shape(shape, [axis], [lo], [hi]) for axis, lo, hi in zip(axes, los, his)]
     if outs is None:
         outs = [pinned_empty(s, x.dtype) for s in out_shapes]
     for o, s in zip(outs, out_shapes):
@@ -872,26 +867,8 @@ def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, 
     if not 2 <= len(specs) <= 3:
         raise ValueError("stencil_multi fuses 2 or 3 axes")
     shape = list(x.shape)
-    out_shape = list(shape)
-    axes, opc, los, his, bcs, fills = [], [], [], [], [], []
-    for axis, op, lo, hi, padding, fill in specs:
-        axis = _norm_axis(axis, x.ndim)
-        if op not in _capi.OPS:
-            raise ValueError(f"unknown op {op!r}")
-        if padding not in ("periodic", "fill", "extend", None):
-            raise NotImplementedError(f"fused multi-axis stencils support periodic / fill / extend, not {padding!r}")
-        if (lo or hi) and padding is None:
-            raise ValueError("no boundary condition was specified but the operation needs to pad the axis")
-        axes.append(axis)
-        opc.append(_capi.OPS[op])
-        los.append(int(lo))
-        his.append(int(hi))
-        bcs.append(_capi.BCS[padding] if (lo or hi) else 0)
-        fills.append(float(fill))
-        out_shape[axis] = shape[axis] + lo + hi - 1
-    if len(set(axes)) != len(axes):
-        raise ValueError("each axis may appear only once")
-    out = pinned_empty(out_shape, x.dtype)
+    axes, opc, los, his, bcs, fills = _stencil_specs(specs, x.ndim, fused=True)
+    out = pinned_empty(_multi_out_shape(shape, axes, los, his), x.dtype)
     n = len(specs)
     IntArr, DblArr = C.c_int * n, C.c_double * n
     dev = host_device_arg(device)
@@ -909,8 +886,7 @@ def cumscan_host(x: np.ndarray, axis: int, reverse: bool = False, trim: str = "n
                  device: HostDevice = None) -> np.ndarray:
     """Host twin of :func:`cumscan` (``xg_cumscan_host``): slabs of a non-operated dim stream through the GPU."""
     lib = _capi.load()
-    if padding not in _capi.BCS:
-        raise ValueError(f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {padding}")
+    _check_padding(padding)
     x, shape, axis, out, pre_op, post_op, dev = _host_scan_prep(x, axis, trim, pad_lo, pad_hi, pre, post, device)
     if out.size:
         rc = lib.xg_cumscan_host(
@@ -1073,13 +1049,8 @@ def vinterp_conservative_host(phi: np.ndarray, theta: np.ndarray, target_bins: n
     if theta.ndim == phi.ndim and theta.shape[axis] != tshape[axis]:
         what = "cell-centre values" if theta_at_centers else "cell bounds"
         raise ValueError(f"theta needs {tshape[axis]} {what} along the axis, got {theta.shape[axis]}")
-    diffs = target_bins[1:] - target_bins[:-1]
-    if bool((diffs < 0).all()):  # transform.py:167-176
-        flip, bins = 1, np.ascontiguousarray(target_bins[::-1])
-    elif bool((diffs > 0).all()):
-        flip, bins = 0, np.ascontiguousarray(target_bins)
-    else:
-        raise ValueError("Target values are not monotonic")
+    flip = _bins_order(target_bins[1:] - target_bins[:-1])
+    bins = np.ascontiguousarray(target_bins[::-1] if flip else target_bins)
     kt, th_ptr, th_st = _host_operand(theta, tshape, phi.dtype, "theta")
     m = int(bins.size)
     out_shape = [s for d, s in enumerate(shape) if d != axis] + [m - 1]

@@ -229,6 +229,17 @@ def _strip_all_coords(data):
     return data.drop_vars(list(data.coords))
 
 
+def missing_boundary_error(ax_name) -> ValueError:
+    """The error of an operator that has to pad ``ax_name`` when no boundary condition is set for it."""
+    return ValueError(
+        f"No boundary condition was specified for axis {ax_name!r}, but the "
+        f"requested operation needs to pad it. Set a boundary condition, "
+        f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
+        f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
+        f"grid method."
+    )
+
+
 def _pad_basic(da: DataArray, grid, padding_width, padding, fill_value):
     from . import ops
     from .device import as_device_tensor, result_like
@@ -241,13 +252,7 @@ def _pad_basic(da: DataArray, grid, padding_width, padding, fill_value):
         _, dim = axis._get_position_name(out)
         ax_padding = padding[ax]
         if ax_padding is None:
-            raise ValueError(
-                f"No boundary condition was specified for axis {ax!r}, but the "
-                f"requested operation needs to pad it. Set a boundary condition, "
-                f"e.g. ``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                f"grid method."
-            )
+            raise missing_boundary_error(ax)
         x, was_host = as_device_tensor(out.data, grid._device_for(out))
         fv = fill_value[ax] if fill_value[ax] is not None else 0.0
         y = ops.pad(x, out.get_axis_num(dim), int(widths[0]), int(widths[1]), ax_padding, fv)
