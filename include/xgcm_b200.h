@@ -356,6 +356,39 @@ XG_API int xg_stencil2_host_connected(int op, int dtype, const void* in, const v
                                       const int64_t* src_strides, const int* negate, int device);
 
 /*
+ * A multi-axis diff / interp / min / max of a HOST field on the two grid topologies whose halo is not a boundary
+ * condition: `nstage` (2 or 3) stencils along distinct dims, one after another, bit for bit the device route's
+ * per-axis launches.  Stage s is xg_stencil2(op[s], axis[s], lo[s], hi[s], bc[s], fill[s]) of its input: the field
+ * for stage 0, the previous stage's result after it (its shape follows from `shape` and the earlier stages'
+ * lo + hi - 1); the last stage writes `out`.  The slab pipeline of xg_stencil2_host_fold / _connected: dim 0 is cut
+ * into slabs and must be a batch dim, operated by no stage and holding no seam (XG_EINVAL).  Per slab, each stage
+ * builds its halo planes from its own input, then runs one xg_stencil2 launch into workspace scratch (two
+ * intermediates, ping-pong) or the result slab; the slabs are sized with the intermediates and the planes for the
+ * largest stage, so device memory stays bounded by the slab size.  Every argument is checked, per stage against
+ * that stage's input shape, before any CUDA call.
+ *
+ * _fold: stage s with fold[s] = 1 crosses a north fold along axis[s] (hi[s] must be 1): one xg_fold_rows launch
+ * (width 1; seam_axis[s], skip[s], mirror[s], period[s] as there, for the stage's input) writes halo_hi, which is
+ * halo_lo too under lo[s] = 1 and bc[s] = XG_BC_PERIODIC.  Other stages pad with bc[s].  XG_ENOTIMPL where
+ * xg_fold_rows would return it.
+ *
+ * _connected: the halo planes of stage s are written by its copy list, as in xg_stencil2_host_connected (no
+ * partner; source 2 reads fill[s]) and described for that stage's whole input; the ncopies[s] copies of the stages
+ * are concatenated in side .. negate (the shapes and strides copy_ndim values per copy).  There is no bc: the copies
+ * cover the unconnected edges too.
+ */
+XG_API int xg_stencil_chain_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                      int nstage, const int* axis, const int* op, const int* lo, const int* hi,
+                                      const int* bc, const double* fill, const int* fold, const int* seam_axis,
+                                      const int* skip, const int64_t* mirror, const int64_t* period, int device);
+XG_API int xg_stencil_chain_host_connected(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                           int nstage, const int* axis, const int* op, const int* lo, const int* hi,
+                                           const double* fill, const int* ncopies, int copy_ndim, const int* side,
+                                           const int* source, const int64_t* dst_offset, const int64_t* src_offset,
+                                           const int64_t* shapes, const int64_t* dst_strides,
+                                           const int64_t* src_strides, const int* negate, int device);
+
+/*
  * Host-buffer twins of xg_stencil_pair: same semantics, HOST pointers, `device` instead of a stream;
  * synchronous.  The slab pipeline of xg_stencil2_host: `a` is cut into slabs along dim 0, `b` streams
  * beside it slab by slab, pre_a / pre_b / post are uploaded whole.  Dim 0 must be a batch dim: not axis_b
@@ -395,7 +428,7 @@ XG_API int xg_host_workspace_bytes(int device, int64_t* bytes);
  * cudaGetDeviceCount.  Groups live for the process.
  *
  * Every *_host entry point that streams slabs (xg_stencil2_host and its _multi / _fold / _connected variants,
- * xg_stencil_multi_host, xg_stencil_pair_host[_fold], xg_cumscan_host, xg_wreduce_host[_multi] and both
+ * xg_stencil_chain_host_fold / _connected, xg_stencil_multi_host, xg_stencil_pair_host[_fold], xg_cumscan_host, xg_wreduce_host[_multi] and both
  * xg_vinterp_*_host) takes a handle in its `device` argument.  The result rows along the call's slab dim are cut
  * into contiguous near-equal blocks, one per member (fewer when there are fewer rows), and each member streams
  * its block on its own host thread through its own workspace, with the whole-call operands uploaded once per

@@ -1,13 +1,16 @@
 """Numpy fields on face-connected and north-fold grids through the host slab pipelines, beside the plain-grid
 host call on the same shape (the ceiling: same slabs, no halo stage) and beside the old whole-field route
 (upload, device call, download): Grid.diff, and Grid.cumsum across the faces (X to outer: a trimmed shift such as
-X to left raises across the cubed sphere's axis-swapping seams), along Z, and reversed across the fold.
+X to left raises across the cubed sphere's axis-swapping seams), along Z, and reversed across the fold; and the
+multi-axis chains, Grid.diff(["X", "Y"]) across the faces and Grid.interp(["X", "Y"]) across the fold, beside the
+same call on a plain grid (xg_stencil_multi_host, one fused launch per slab), the old route and the single-axis
+streamed call.
 Page-locked inputs, host clock around each synchronous call, the variants alternated `--rounds` times in one
 process.  Prints one JSON line with the card, its power limit, the median seconds and GB/s (bytes in + out over
 time) of every variant, its ratio to the plain-grid ceiling and to the old route, and tools/bench_pcie.py's copy
 rates.
 
-    python tools/bench_host_halo.py [--faces 90 6 2160 2160] [--fold 75 3059 4322] [--rounds 5]
+    python tools/bench_host_halo.py [--faces 90 6 2160 2160] [--fold [T] 75 3059 4322] [--rounds 5]
 
 If MemAvailable allows about 2.2x of it, a year of monthly ORCA12-like temperature (12, 75, 3059, 4322) fp32
 (47.6 GB) also streams across the fold (diff, then the reverse cumsum), with sampled time steps checked against
@@ -107,8 +110,11 @@ def faces_variants(shape):
         "plain_cumsumX": lambda: plain.cumsum(xg.DataArray(c, dims=cd), "X", to="outer"),
         "faces_cumsumZ": lambda: grid.cumsum(xg.DataArray(c, dims=cd), "Z", padding="fill"),
         "plain_cumsumZ": lambda: plain.cumsum(xg.DataArray(c, dims=cd), "Z"),
+        "faces_diffXY": lambda: grid.diff(xg.DataArray(c, dims=cd), ["X", "Y"], padding="fill"),
+        "plain_diffXY": lambda: plain.diff(xg.DataArray(c, dims=cd), ["X", "Y"]),
     }
-    if fits:
+    if fits:  # input, intermediate, result
+        variants["faces_diffXY_old"] = old_route(grid, "diff", c, cd, axis=["X", "Y"], padding="fill")
         variants["faces_scalar_diffX_old"] = old_route(grid, "diff", c, cd, axis="X", padding="fill")
         variants["faces_vector_diffX_old"] = old_route(grid, "diff", c, ud, {"Y": (v, vd)}, axis="X", padding="fill")
     if 4 * c.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:  # input, scan, padded copy, result
@@ -133,6 +139,8 @@ def fold_variants(shape):
     a = pinned_random(shape, 3)
     dims = ("t", "z", "yl", "xc")[-len(shape):]
     variants = {
+        "fold_interpXY": lambda: grid.interp(xg.DataArray(a, dims=dims), ["X", "Y"], to={"Y": "center"}),
+        "plain_fold_shape_interpXY": lambda: plain.interp(xg.DataArray(a, dims=dims), ["X", "Y"], to={"Y": "center"}),
         "fold_diffY": lambda: grid.diff(xg.DataArray(a, dims=dims), "Y", to="center"),
         "plain_fold_shape_diffY": lambda: plain.diff(xg.DataArray(a, dims=dims), "Y", to="center"),
         "fold_cumsumY_reverse": lambda: grid.cumsum(xg.DataArray(a, dims=dims), "Y", to="center", reverse=True),
@@ -141,6 +149,8 @@ def fold_variants(shape):
     }
     if 2 * a.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:
         variants["fold_diffY_old"] = old_route(grid, "diff", a, dims, axis="Y", to="center")
+    if 3 * a.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:  # input, intermediate, result
+        variants["fold_interpXY_old"] = old_route(grid, "interp", a, dims, axis=["X", "Y"], to={"Y": "center"})
     if 4 * a.nbytes < 0.8 * torch.cuda.mem_get_info()[0]:  # input, scan, padded copy, result
         variants["fold_cumsumY_reverse_old"] = old_route(grid, "cumsum", a, dims, axis="Y", to="center", reverse=True)
     return variants, 2 * a.nbytes, {}
@@ -216,11 +226,15 @@ def main():
     for name, ceiling in (("faces_scalar_diffX", "plain_diffX"), ("faces_vector_diffX", "plain_diffX"),
                           ("fold_diffY", "plain_fold_shape_diffY"), ("faces_cumsumX", "plain_cumsumX"),
                           ("faces_cumsumZ", "plain_cumsumZ"),
-                          ("fold_cumsumY_reverse", "plain_fold_shape_cumsumY_reverse")):
+                          ("fold_cumsumY_reverse", "plain_fold_shape_cumsumY_reverse"),
+                          ("faces_diffXY", "plain_diffXY"), ("fold_interpXY", "plain_fold_shape_interpXY")):
         if name in result and ceiling in result:
             result[name]["vs_plain"] = result[name]["s"] / result[ceiling]["s"]
         if name in result and name + "_old" in result:
             result[name]["vs_old"] = result[name]["s"] / result[name + "_old"]["s"]
+    for name, single in (("faces_diffXY", "faces_scalar_diffX"), ("fold_interpXY", "fold_diffY")):
+        if name in result and single in result:
+            result[name]["vs_single_axis"] = result[name]["s"] / result[single]["s"]
     result["orca_year"] = {"skipped": "--skip-year"} if args.skip_year else orca_year(args.rounds)
     print(json.dumps(result))
 

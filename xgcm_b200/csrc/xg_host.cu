@@ -26,7 +26,10 @@
 // second streamed input, and each slab is one xg_stencil_pair_halo launch (after the xg_fold_rows launch of b's
 // folded row, for the fold).  xg_cumscan_host_fold / xg_cumscan_host_connected run the same halo stages on each
 // slab's scanned rows (xg_cumscan into the scratch buffer), then place the scanned slab and its halo planes into the
-// padded result slab and divide by the post-metric.
+// padded result slab and divide by the post-metric.  xg_stencil_chain_host_fold / _connected run a multi-axis
+// diff / interp / min / max as the device route does, one axis after another: per slab, each stage builds its halo
+// planes from its own input (the slab input, or the previous stage's result in the scratch buffer) and runs one
+// xg_stencil2 launch into the next intermediate or the result slab.
 #include <stdlib.h>
 
 #include <thread>
@@ -797,6 +800,94 @@ int cumscan_halo_host(const char* who, const ScanCall& s, const int64_t* scan_sh
   });
 }
 
+// ---------------------------------------------------------------------------------- the chain entry points
+// The checks both chain entry points share, before any CUDA call: stage count, pointers, in-place, and per stage
+// (cs[s], whose shape is shapes[s]) those of a halo stencil plus its op and distinct axes.  Fills shapes[0 ..
+// nstage] (the result's shape last); cs[s].shape points at shapes[s].
+int validate_chain(const char* who, int dtype, const void* in, void* out, int ndim, const int64_t* shape, int nstage,
+                   const int* axis, const int* op, const int* lo, const int* hi, const int* bc, const double* fill,
+                   int device, Call* cs, int64_t (*shapes)[XG_MAX_NDIM]) {
+  const std::string w(who);
+  if (!in || !out || !shape || !axis || !op || !lo || !hi || !fill) return xg_fail(XG_EINVAL, w + ": null pointer");
+  if (nstage < 2 || nstage > 3) return xg_fail(XG_EINVAL, w + ": a chain has 2 or 3 stages");
+  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, w + ": bad ndim");
+  if (in == out) return xg_fail(XG_EINVAL, w + ": in-place operation is not supported");
+  for (int d = 0; d < ndim; ++d) shapes[0][d] = shape[d];
+  for (int s = 0; s < nstage; ++s) {
+    const int b = bc ? bc[s] : ((lo[s] || hi[s]) ? XG_BC_FILL : XG_BC_NONE);  // connected: the planes pad
+    cs[s] = Call{op[s], dtype, in, out, ndim, shapes[s], axis[s], lo[s], hi[s], b, fill[s],
+                 nullptr, nullptr, nullptr, nullptr, device};
+    int rc = validate_halo_call(who, cs[s]);
+    if (rc) return rc;
+    if (op[s] < XG_OP_DIFF || op[s] > XG_OP_MAX) return xg_fail(XG_EINVAL, w + ": unknown op");
+    for (int k = 0; k < s; ++k)
+      if (axis[k] == axis[s]) return xg_fail(XG_EINVAL, w + ": each axis may appear only once");
+    for (int d = 0; d < ndim; ++d) shapes[s + 1][d] = shapes[s][d];
+    shapes[s + 1][axis[s]] += lo[s] + hi[s] - 1;
+  }
+  return XG_OK;
+}
+
+// A chain entry point (arguments checked) on cs[0].device: the field in slabs along dim 0 and, per slab, the
+// per-axis launch sequence of the device route: stage s builds its halo planes from its own input (`halo[s]`, empty
+// for none) and runs one xg_stencil2 into the intermediate it writes (scratch, ping-pong) or the result slab.
+// `fill_host`: the stages' fill constants (nstage elements of the field's dtype) the copy lists read, or nullptr.
+int chain_host(const char* who, const Call* cs, const HaloFn* halo, int nstage, const int64_t (*shapes)[XG_MAX_NDIM],
+               const void* fill_host) {
+  const Call& c0 = cs[0];
+  const size_t es = c0.dtype == XG_F32 ? 4 : 8;
+  const int ndim = c0.ndim;
+  const View3 vin = view3(ndim, shapes[0], 0), vout = view3(ndim, shapes[nstage], 0);
+  int64_t mid[2] = {0, 0};  // elements per dim-0 row of the intermediates (stage 0's and stage 1's results)
+  PipeExtra ex;
+  for (int s = 0; s < nstage; ++s) {
+    if (s + 1 < nstage) mid[s] = view3(ndim, shapes[s + 1], 0).R;
+    const int64_t n = shapes[s][cs[s].axis];
+    const size_t plane = n ? (size_t)(view3(ndim, shapes[s], 0).R / n) * es : 0;
+    if (halo[s] && plane > ex.plane_row_bytes) ex.plane_row_bytes = plane;  // planes sized for the largest stage
+  }
+  ex.scratch_row_bytes = (size_t)(mid[0] + mid[1]) * es;
+  ex.row_bytes = (vin.R + vout.R) * (int64_t)es + (int64_t)ex.scratch_row_bytes;  // the slab counts them all
+  return spread(who, c0.device, vout.L, false, [&](int device, int64_t r0, int64_t r1) -> int {
+    Session ss;
+    int rc = ss.open(device);
+    if (rc) return rc;
+    if (vout.L <= 0 || vout.R == 0 || vin.R == 0) return XG_OK;
+    const void* d_fill = nullptr;
+    rc = ss.upload(kAuxFill, fill_host, (size_t)nstage * es, &d_fill);
+    if (rc == XG_OK) rc = ss.fence();
+    if (rc) return rc;
+    auto launch = [&](int64_t j0, int64_t j1, int64_t, int64_t, const SlabBufs& b, cudaStream_t st) -> int {
+      char* scratch = static_cast<char*>(b.scratch);
+      void* mids[2] = {scratch, scratch + (size_t)((j1 - j0) * mid[0]) * es};
+      const void* src = b.in;
+      for (int s = 0; s < nstage; ++s) {
+        const Call& c = cs[s];
+        int64_t sshape[XG_MAX_NDIM];
+        for (int d = 0; d < ndim; ++d) sshape[d] = shapes[s][d];
+        sshape[0] = j1 - j0;
+        const void *hl = nullptr, *hh = nullptr;
+        if (halo[s]) {
+          SlabBufs sb = b;  // the halo stages read b.in: point it at this stage's input
+          sb.in = const_cast<void*>(src);
+          const void* f = d_fill ? static_cast<const char*>(d_fill) + (size_t)s * es : nullptr;
+          int rc2 = halo[s](sb, sshape, nullptr, f, st, &hl, &hh);
+          if (rc2) return rc2;
+        }
+        void* dst = s + 1 == nstage ? b.out[0] : mids[s];
+        int rc2 = xg_stencil2(c.op, c.dtype, src, dst, ndim, sshape, c.axis, c.lo, c.hi,
+                              (c.lo || c.hi) ? c.bc : XG_BC_NONE, c.fill_value, nullptr, nullptr, nullptr, nullptr,
+                              hl, hh, st);
+        if (rc2) return rc2;
+        src = dst;
+      }
+      return XG_OK;
+    };
+    void* outs[1] = {c0.out};
+    return ss.run(es, c0.in, vin, 1, outs, &vout, launch, ex.rows(r0, r1));
+  });
+}
+
 }  // namespace
 }  // namespace xg_host
 
@@ -957,6 +1048,68 @@ extern "C" int xg_cumscan_host_connected(int dtype, const void* in, void* out, i
   const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
   const void* fill_host = fill ? (dtype == XG_F32 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
   return cumscan_halo_host(who, s, scan_shape, copy_stage(cl, dtype, pad_lo, pad_hi), fill_host);
+}
+
+extern "C" int xg_stencil_chain_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                          int nstage, const int* axis, const int* op, const int* lo, const int* hi,
+                                          const int* bc, const double* fill, const int* fold, const int* seam_axis,
+                                          const int* skip, const int64_t* mirror, const int64_t* period, int device) {
+  const char* who = "xg_stencil_chain_host_fold";
+  if (!bc || !fold || !seam_axis || !skip || !mirror || !period)
+    return xg_fail(XG_EINVAL, std::string(who) + ": null pointer");
+  Call cs[3];
+  int64_t shapes[4][XG_MAX_NDIM];
+  int rc = validate_chain(who, dtype, in, out, ndim, shape, nstage, axis, op, lo, hi, bc, fill, device, cs, shapes);
+  if (rc) return rc;
+  HaloFn halo[3];
+  for (int s = 0; s < nstage; ++s) {
+    if (fold[s] != 0 && fold[s] != 1) return xg_fail(XG_EINVAL, std::string(who) + ": fold must be 0 or 1");
+    if (!fold[s]) continue;
+    rc = validate_fold(who, cs[s], seam_axis[s], skip[s], mirror[s], period[s]);
+    if (rc) return rc;
+    halo[s] = fold_stage(cs[s], false, seam_axis[s], skip[s], mirror[s], period[s], 0);
+  }
+  return chain_host(who, cs, halo, nstage, shapes, nullptr);
+}
+
+extern "C" int xg_stencil_chain_host_connected(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                               int nstage, const int* axis, const int* op, const int* lo,
+                                               const int* hi, const double* fill, const int* ncopies, int copy_ndim,
+                                               const int* side, const int* source, const int64_t* dst_offset,
+                                               const int64_t* src_offset, const int64_t* shapes,
+                                               const int64_t* dst_strides, const int64_t* src_strides,
+                                               const int* negate, int device) {
+  const std::string who = "xg_stencil_chain_host_connected";
+  if (!ncopies) return xg_fail(XG_EINVAL, who + ": null pointer");
+  Call cs[3];
+  int64_t sh[4][XG_MAX_NDIM];
+  int rc = validate_chain(who.c_str(), dtype, in, out, ndim, shape, nstage, axis, op, lo, hi, nullptr, fill, device,
+                          cs, sh);
+  if (rc) return rc;
+  HaloFn halo[3];
+  bool any_fill = false;
+  int64_t k0 = 0;  // the first copy of stage s in the concatenated lists
+  for (int s = 0; s < nstage; ++s) {
+    const size_t k = (size_t)k0, kd = (size_t)k0 * (size_t)(copy_ndim > 0 ? copy_ndim : 0);
+    const CopyList cl{ncopies[s], copy_ndim, side ? side + k : nullptr, source ? source + k : nullptr,
+                      dst_offset ? dst_offset + k : nullptr, src_offset ? src_offset + k : nullptr,
+                      shapes ? shapes + kd : nullptr, dst_strides ? dst_strides + kd : nullptr,
+                      src_strides ? src_strides + kd : nullptr, negate ? negate + k : nullptr};
+    int64_t row_in = 1;
+    for (int d = 1; d < ndim; ++d) row_in *= sh[s][d];
+    const int64_t plane_row = sh[s][axis[s]] ? row_in / sh[s][axis[s]] : 0;
+    bool fill_s = false;
+    rc = validate_copies(who + ": stage " + std::to_string(s), cl, lo[s], hi[s], sh[s][0], plane_row, row_in, false,
+                         0, &fill_s);
+    if (rc) return rc;
+    any_fill = any_fill || fill_s;
+    if (lo[s] || hi[s]) halo[s] = copy_stage(cl, dtype, lo[s], hi[s]);
+    k0 += cl.n;
+  }
+  float f32[3];
+  for (int s = 0; s < nstage; ++s) f32[s] = (float)fill[s];  // pageable: staged before cudaMemcpyAsync returns
+  const void* fill_host = any_fill ? (dtype == XG_F32 ? (const void*)f32 : (const void*)fill) : nullptr;
+  return chain_host(who.c_str(), cs, halo, nstage, sh, fill_host);
 }
 
 extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,

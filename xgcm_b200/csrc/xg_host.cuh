@@ -22,7 +22,7 @@ enum Aux {
   kAuxPreA,         // pre-metric of a pair's x term
   kAuxWrapLo,       // periodic wrap plane below the first slab of dim 0 (plane n0 - 1)
   kAuxWrapHi,       // ... and above the last one (plane 0)
-  kAuxFill,         // fill constant the unconnected face edges copy from
+  kAuxFill,         // fill constant the unconnected face edges copy from (one per stage of a chain)
   kAuxTheta,        // a broadcast theta
   kAuxThetaBounds,  // its bounds, made on the device from centres
   kAuxTarget,       // target levels of xg_vinterp_linear_host, or the bins of xg_vinterp_conservative_host

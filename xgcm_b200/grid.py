@@ -573,6 +573,8 @@ class Grid:
             and set(kwargs) <= {"padding", "fill_value"}
         ):
             fused = self._fused_multi_axis(funcname, array, axis, to, kwargs)
+            if fused is None and other_component is None:  # a scalar field: no vector halo across a seam
+                fused = self._multi_axis_halo_host(funcname, array, axis, to, kwargs)
             if fused is not None:
                 return self._wrap_out(fused, as_xarray)
         if host_input and n_axes > 1:
@@ -642,6 +644,80 @@ class Grid:
         out_dims = tuple(rename.get(d, d) for d in array.dims)
         res = DataArray(out, dims=out_dims, name=array.name, attrs=array.attrs)
         return _reattach_coords([res], self, None, set(rename.values()), [array])[0]
+
+    def _multi_axis_halo_host(self, funcname, array, axis, to, kwargs):
+        """A multi-axis diff / interp / min / max of a numpy field on a face-connected grid, or across a north fold,
+        streamed through the GPU in slabs (``xg_stencil_chain_host_connected`` / ``_fold``) instead of uploaded
+        whole: per slab, the device route's per-axis launches in the order given, each stage's halo planes built
+        from its own input, so the values are those of the device route.  Each stage is resolved against the
+        intermediate's dims and shape, and its errors are raised before anything streams.  Returns the result, or
+        None for the whole-field route: no face connection and no folded term, a device array, no CUDA device, a
+        boundary the halo stencils do not take (extrapolate), no batch dim in front of the operated, seam and face
+        dims (``_host_stream_route``), a fold the plan cannot mirror."""
+        from . import ops
+        from .padding import _axis_dim, _fold_plan, connected_halo_program
+
+        connected = self._face_connections is not None
+        if not (connected or self._folds) or not _is_host_float(array) or self._device_for(array).type != "cuda":
+            return None
+        padding, fill_value = kwargs.get("padding"), kwargs.get("fill_value")
+        paddings = self._complete_user_kwargs_using_axis_defaults(padding, "padding")
+        fills = self._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
+        if connected:  # every padded edge takes its value from connected_edge_mode below, which raises its own errors
+            paddings = {k: "fill" if v is None else v for k, v in paddings.items()}
+        dims, shape = tuple(array.dims), [int(v) for v in array.shape]
+        stages = []  # (term, the stage's input dims and shape, edge mode and fill of a connected stage)
+        probe = DataArray.__new__(DataArray)
+        for ax_name in axis:
+            probe._dims = dims
+            t = _stencil_term(self, funcname, probe, ax_name, to.get(ax_name), paddings, fills)
+            mode = None
+            if connected:
+                mode = connected_edge_mode(self, ax_name, t.lo, t.hi, padding, fill_value,
+                                           shape[dims.index(self._facedim)])
+            elif t.pad_mode not in ("periodic", "fill", "extend", None):
+                return None  # e.g. the opt-in extrapolate extension
+            stages.append((t, dims, shape, mode))
+            dims = tuple(t.out_dim if d == t.in_dim else d for d in dims)
+            shape = list(shape)
+            shape[t.axis_num] += t.lo + t.hi - 1
+        if not connected and not any(t.folded for t, *_ in stages):
+            return None
+        in_dims = stages[0][1]
+        core = [t.in_dim for t, *_ in stages]
+        if connected:
+            core += [self._facedim] + [d for a in _get_all_connection_axes(self._face_connections, self._facedim)
+                                       for d in self.axes[a].coords.values() if d in in_dims]
+        else:
+            core.append(_axis_dim(self, in_dims, self._folds[next(t for t, *_ in stages if t.folded).ax_name]
+                                  ["seam_axis"]))
+        cut = _host_stream_route("connected" if connected else "fold", in_dims, stages[0][2], core,
+                                 max(t.lo for t, *_ in stages), max(t.hi for t, *_ in stages))
+        if cut is None:
+            return None
+        specs, programs = [], []
+        for t, s_dims, s_shape, mode in stages:
+            m_dims, m_shape = cut.dims(s_dims), cut.shape(s_shape)
+            if connected:
+                specs.append((cut.axis(t.axis_num), funcname, t.lo, t.hi, mode[1]))
+                programs.append(connected_halo_program(self, t.ax_name, t.lo, t.hi, m_dims, m_shape, mode[0]))
+                continue
+            plan = None
+            if t.folded:
+                try:
+                    _, seam, skip, mirror, period = _fold_plan(self, t.ax_name, m_dims, m_shape, 1)
+                except NotImplementedError:
+                    return None
+                plan = (seam, skip, mirror, period)
+            specs.append((cut.axis(t.axis_num), funcname, t.lo, t.hi, t.pad_mode if (t.lo or t.hi) else None, t.fill,
+                          plan))
+        x, device = cut.cut(array.data), self._host_device(array)
+        if connected:
+            y = ops.stencil_chain_host_connected(x, specs, programs, device=device)
+        else:
+            y = ops.stencil_chain_host_fold(x, specs, device=device)
+        res = DataArray(y.reshape(shape), dims=dims, name=array.name, attrs=array.attrs)
+        return _reattach_coords([res], self, None, {t.out_dim for t, *_ in stages}, [array])[0]
 
     def apply_many(self, da, requests, padding=None, fill_value=None):
         """Several single-axis operators of ONE field in one call (an extension; the reference has no

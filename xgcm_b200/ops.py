@@ -715,6 +715,64 @@ def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int,
     return out
 
 
+def _chain_args(x, specs):
+    """C-ABI values of the stages ``specs`` of a host chain (``_stencil_specs``): the count, the page-locked result,
+    the int arrays of axes, op codes, lo and hi, the boundary codes, and the fills."""
+    import ctypes as C
+
+    n = len(specs)
+    axes, opc, los, his, bcs, fills = _stencil_specs(specs, x.ndim, fused=False)
+    out = pinned_empty(_multi_out_shape(list(x.shape), axes, los, his), x.dtype)
+    i32 = C.c_int * max(n, 1)
+    return n, out, (i32(*axes), i32(*opc), i32(*los), i32(*his)), i32(*bcs), (C.c_double * max(n, 1))(*fills)
+
+
+def stencil_chain_host_fold(x: np.ndarray, stages, device: HostDevice = None) -> np.ndarray:
+    """A multi-axis stencil of a host field on a fold grid, stage by stage as the device route launches it
+    (``xg_stencil_chain_host_fold``).  ``stages``: 2 or 3 of ``(axis, op, lo, hi, padding, fill, fold)``, each on the
+    previous stage's result, ``fold`` None or ``(seam_axis, skip, mirror, period)`` (:func:`fold_rows`, planned for
+    that stage's input) when the stage's north edge crosses the fold.  Dim 0 is cut into slabs and must be a batch
+    dim."""
+    import ctypes as C
+
+    lib = _capi.load()
+    x = _host_field(x, "stencil_chain_host_fold: field", cast=False)
+    n, out, (axes, opc, los, his), bcs, fills = _chain_args(x, [s[:6] for s in stages])
+    plans = [s[6] if s[6] is not None else (0, 0, 0, 1) for s in stages]
+    i32 = C.c_int * max(n, 1)
+    if out.size:
+        rc = lib.xg_stencil_chain_host_fold(
+            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(x.shape), n, axes,
+            opc, los, his, bcs, fills, i32(*[0 if s[6] is None else 1 for s in stages]),
+            i32(*[_norm_axis(p[0], x.ndim) for p in plans]), i32(*[int(p[1]) for p in plans]),
+            _capi.i64_array([p[2] for p in plans]), _capi.i64_array([p[3] for p in plans]), host_device_arg(device))
+        _capi.check(rc)
+    return out
+
+
+def stencil_chain_host_connected(x: np.ndarray, stages, programs, device: HostDevice = None) -> np.ndarray:
+    """:func:`stencil_chain_host_fold` on a grid with face connections (``xg_stencil_chain_host_connected``):
+    ``stages`` of ``(axis, op, lo, hi, fill)``; ``programs[s]`` writes the halo planes of stage ``s``, the copy list
+    of :func:`stencil2_host_connected` (``padding.connected_halo_program``) for that stage's input, sources "self"
+    and "fill" (``fill`` of the stage)."""
+    import ctypes as C
+
+    lib = _capi.load()
+    x = _host_field(x, "stencil_chain_host_connected: field", cast=False)
+    if len(programs) != len(stages):
+        raise ValueError("stencil_chain_host_connected: one halo program per stage")
+    specs = [(axis, op, lo, hi, "fill" if (lo or hi) else None, fill) for axis, op, lo, hi, fill in stages]
+    n, out, (axes, opc, los, his), _, fills = _chain_args(x, specs)
+    _, cndim, side, source, doff, soff, shapes, dstr, sstr, neg = _copy_list_args([c for p in programs for c in p])
+    if out.size:
+        rc = lib.xg_stencil_chain_host_connected(
+            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(x.shape), n, axes,
+            opc, los, his, fills, (C.c_int * max(n, 1))(*[len(p) for p in programs]), cndim, side, source, doff, soff,
+            shapes, dstr, sstr, neg, host_device_arg(device))
+        _capi.check(rc)
+    return out
+
+
 def _pair_specs(spec_a, spec_b, ndim: int):
     """C-ABI values of the two terms of a pair: ``(op_a, lo_a, hi_a, bc_a, fill_a)``, ``(axis_b, op_b, lo_b, hi_b,
     bc_b, fill_b)``."""
