@@ -1,5 +1,6 @@
-"""The C-ABI of the multi-axis host twins without a GPU: xg_stencil_multi_host and xg_wreduce_host_multi are
-exported and check every argument before any CUDA call (a CUDA call here would fail with XG_ECUDA)."""
+"""The C-ABI of the multi-result and multi-axis host twins without a GPU: xg_stencil2_host_multi,
+xg_stencil_multi_host and xg_wreduce_host_multi check every argument before any CUDA call (a CUDA call here would
+fail with XG_ECUDA); the two multi-axis twins are exported."""
 
 import ctypes as C
 
@@ -70,6 +71,52 @@ def test_stencil_multi_host_checks_arguments_without_gpu(lib):
         assert _capi.last_error().startswith("xg_stencil_multi_host: ")
     # an empty result returns before the device is touched
     assert call(shp=_capi.i64_array([0, 4, 4])) == 0
+
+
+def test_stencil2_host_multi_checks_arguments_without_gpu(lib):
+    buf = (C.c_float * 64)()
+    res = [(C.c_float * 64)() for _ in range(2)]
+    outs = (C.c_void_p * 2)(*[C.addressof(r) for r in res])
+    shape = _capi.i64_array([4, 4, 4])
+    fills = (C.c_double * 2)(0.0, 0.0)
+
+    def call(nout=2, ops=_ints(0, 1), dtype=0, src=buf, dst=outs, ndim=3, shp=shape, axes=_ints(2, 0),
+             lo=_ints(1, 1), hi=_ints(0, 0), bc=_ints(1, 2), fill=fills):
+        return lib.xg_stencil2_host_multi(nout, ops, dtype, src, dst, ndim, shp, axes, lo, hi, bc, fill, 0)
+
+    cases = [
+        (dict(src=None), EINVAL, "null pointer"),
+        (dict(dst=None), EINVAL, "null pointer"),
+        (dict(shp=None), EINVAL, "null pointer"),
+        (dict(ops=None), EINVAL, "null pointer"),
+        (dict(axes=None), EINVAL, "null pointer"),
+        (dict(lo=None), EINVAL, "null pointer"),
+        (dict(hi=None), EINVAL, "null pointer"),
+        (dict(bc=None), EINVAL, "null pointer"),
+        (dict(fill=None), EINVAL, "null pointer"),
+        (dict(nout=0), EINVAL, "between 1 and 8 results per call"),
+        (dict(nout=9), EINVAL, "between 1 and 8 results per call"),
+        (dict(dst=(C.c_void_p * 2)(outs[0], None)), EINVAL, "null result pointer"),
+        (dict(dtype=5), EINVAL, "dtype must be XG_F32 or XG_F64"),
+        (dict(ndim=0), EINVAL, "bad ndim"),
+        (dict(ndim=9), EINVAL, "bad ndim"),
+        (dict(axes=_ints(3, 0)), EINVAL, "axis out of range"),
+        (dict(axes=_ints(2, -1)), EINVAL, "axis out of range"),
+        (dict(lo=_ints(2, 1)), EINVAL, "halo widths must be 0 or 1"),
+        (dict(hi=_ints(0, -1)), EINVAL, "halo widths must be 0 or 1"),
+        (dict(bc=_ints(0, 2)), EINVAL, "no boundary condition was specified but the operation needs to pad the axis"),
+        (dict(bc=_ints(1, 5)), EINVAL, "no boundary condition was specified but the operation needs to pad the axis"),
+        (dict(shp=_capi.i64_array([4, 4, 0])), EINVAL, "empty operated axis"),
+        (dict(shp=_capi.i64_array([0, 4, 4])), EINVAL, "empty operated axis"),
+        # dim 0 is cut into slabs: a result along it keeps its extent and pads only at the field's ends
+        (dict(hi=_ints(0, 1)), ENOTIMPL, "outer / inner shifts along the outermost dimension"),
+        (dict(lo=_ints(1, 0)), ENOTIMPL, "outer / inner shifts along the outermost dimension"),
+        (dict(bc=_ints(1, 4)), ENOTIMPL, "extrapolate along the outermost dimension"),
+    ]
+    for kw, rc, msg in cases:
+        assert call(**kw) == rc, kw
+        assert msg in _capi.last_error(), (kw, _capi.last_error())
+        assert _capi.last_error().startswith("xg_stencil2_host_multi: ")
 
 
 def test_wreduce_host_multi_checks_arguments_without_gpu(lib):

@@ -19,6 +19,8 @@
 //
 // The stencil entry points here slab dim 0.  xg_stencil2_host: when dim 0 is the operated axis, consecutive slabs
 // overlap by the one-cell halo and the exterior halo plane (periodic wrap) is uploaded once.
+// xg_stencil2_host_multi: the same with up to kMaxOut results of one uploaded slab, so a `Grid.diff` + `Grid.interp`
+// sweep over X, Y, Z moves the field over PCIe once, not six times; its results along dim 0 keep that extent.
 // xg_stencil2_host_fold / xg_stencil2_host_connected: dim 0 is a batch dim, and a per-slab halo stage on the kernel
 // stream builds the slab's halo_lo / halo_hi planes from the slab buffers (one xg_fold_rows launch, or the
 // face-connection copy list clipped to the slab and replayed with xg_strided_copy_batch) just before its
@@ -144,6 +146,20 @@ View3 view3(int ndim, const int64_t* shape, int sd) {
   for (int d = 0; d < sd; ++d) v.C *= shape[d];
   for (int d = sd + 1; d < ndim; ++d) v.R *= shape[d];
   return v;
+}
+
+int read_window(const char* who, int64_t j0, int64_t j1, int lo, int64_t n, int64_t i0, int64_t i1, Window* w) {
+  *w = Window{j0 - lo, j1 - lo + 1, 0, 0};
+  if (w->s0 < 0) {
+    w->s0 = 0;
+    w->slo = 1;
+  }
+  if (w->s1 > n) {
+    w->s1 = n;
+    w->shi = 1;
+  }
+  if (w->s0 < i0 || w->s1 > i1) return xg_fail(XG_EINVAL, std::string(who) + ": internal slab window error");
+  return XG_OK;
 }
 
 size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size_t es) {
@@ -490,80 +506,100 @@ HaloFn fold_stage(const Call& c, bool of_in2, int seam_axis, int skip, int64_t m
   };
 }
 
-// A stencil entry point (arguments checked) on c.device: field c.in in slabs along dim 0, `partner` (field b of pair
-// `t`, or the partner vector component, `partner_row` elements per dim-0 index) beside it, the metrics (and the
-// `fill_host` constant, es bytes, when given) uploaded whole.  Per slab `halo` (when dim 0 is a batch dim) builds
-// the halo planes, then one xg_stencil2 or xg_stencil_pair_halo launch.
-int stencil_host(const char* who, const Call& c, const PairTerm* t, const void* partner, int64_t partner_row,
-                 const HaloFn& halo, const void* fill_host = nullptr) {
-  const size_t es = c.dtype == XG_F32 ? 4 : 8;
-  const int ndim = c.ndim, lo = c.lo;
-  const bool ax0 = c.axis == 0;
-  const int64_t n0 = c.shape[0];
-  int64_t out_shape[XG_MAX_NDIM];
-  for (int d = 0; d < ndim; ++d) out_shape[d] = c.shape[d];
-  out_shape[c.axis] = c.shape[c.axis] + c.lo + c.hi - 1;
-  const View3 vin = view3(ndim, c.shape, 0), vout = view3(ndim, out_shape, 0);
-  const bool edge_pairs = ax0 && c.bc == XG_BC_EXTRAPOLATE && (lo || c.hi);
-  return spread(who, c.device, vout.L, edge_pairs, [&](int device, int64_t r0, int64_t r1) -> int {
+// A stencil entry point (arguments checked) on cs[0].device: field cs[0].in in slabs along dim 0, into the `nout`
+// results cs[k].out (1 .. kMaxOut), which share in, dtype, ndim, shape and device.  With one result only: `partner`
+// (field b of pair `t`, or the partner vector component, `partner_row` elements per dim-0 index) beside the field,
+// the metrics (and the `fill_host` constant, es bytes, when given) uploaded whole, and per slab `halo` (when dim 0 is
+// a batch dim) building the halo planes.  Per slab, one xg_stencil2 or xg_stencil_pair_halo launch per result.
+int stencil_host(const char* who, int nout, const Call* cs, const PairTerm* t, const void* partner,
+                 int64_t partner_row, const HaloFn& halo, const void* fill_host = nullptr) {
+  const Call& c0 = cs[0];
+  const size_t es = c0.dtype == XG_F32 ? 4 : 8;
+  const int ndim = c0.ndim;
+  const int64_t n0 = c0.shape[0];
+  const View3 vin = view3(ndim, c0.shape, 0);
+  int64_t out_shape[kMaxOut][XG_MAX_NDIM];
+  View3 vout[kMaxOut];
+  bool empty = vin.R == 0, wrap_lo = false, wrap_hi = false;
+  PipeExtra ex;
+  for (int k = 0; k < nout; ++k) {
+    const Call& c = cs[k];
+    for (int d = 0; d < ndim; ++d) out_shape[k][d] = c.shape[d];
+    out_shape[k][c.axis] = c.shape[c.axis] + c.lo + c.hi - 1;
+    vout[k] = view3(ndim, out_shape[k], 0);
+    empty = empty || vout[k].L <= 0 || vout[k].R == 0;
+    if (c.axis != 0) continue;
+    // a slab reads the input rows read_window gives its results along dim 0
+    if (c.lo > ex.lo_rows) ex.lo_rows = c.lo;
+    if (1 - c.lo > ex.hi_rows) ex.hi_rows = 1 - c.lo;
+    ex.edge_pairs = ex.edge_pairs || (c.bc == XG_BC_EXTRAPOLATE && (c.lo || c.hi));
+    wrap_lo = wrap_lo || (c.bc == XG_BC_PERIODIC && c.lo);
+    wrap_hi = wrap_hi || (c.bc == XG_BC_PERIODIC && c.hi);
+  }
+  if (partner) {
+    ex.hin2 = partner;
+    ex.in2 = View3{1, n0, partner_row};
+  }
+  if (halo) ex.plane_row_bytes = (size_t)(vin.R / c0.shape[c0.axis]) * es;
+  return spread(who, c0.device, vout[0].L, ex.edge_pairs, [&](int device, int64_t r0, int64_t r1) -> int {
     Session ss;
     int rc = ss.open(device);
     if (rc) return rc;
-    if (vout.L <= 0 || vout.R == 0 || vin.R == 0) return XG_OK;
+    if (empty) return XG_OK;
 
     const void *d_pre, *d_post, *d_pre_a = nullptr, *d_fill = nullptr;
     const void* wrap[2] = {nullptr, nullptr};  // periodic halo planes along dim 0: plane n0 - 1 below, plane 0 above
     const size_t plane = (size_t)vin.R * es;
-    rc = ss.upload(kAuxPre, c.pre, c.pre ? operand_span(c.pre_strides, c.shape, ndim, es) : 0, &d_pre);
+    rc = ss.upload(kAuxPre, c0.pre, c0.pre ? operand_span(c0.pre_strides, c0.shape, ndim, es) : 0, &d_pre);
     if (rc == XG_OK)
-      rc = ss.upload(kAuxPost, c.post, c.post ? operand_span(c.post_strides, out_shape, ndim, es) : 0, &d_post);
+      rc = ss.upload(kAuxPost, c0.post, c0.post ? operand_span(c0.post_strides, out_shape[0], ndim, es) : 0, &d_post);
     if (rc == XG_OK && t && t->pre_a)
-      rc = ss.upload(kAuxPreA, t->pre_a, operand_span(t->pre_a_strides, c.shape, ndim, es), &d_pre_a);
-    if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && lo)
-      rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
-    if (rc == XG_OK && ax0 && c.bc == XG_BC_PERIODIC && c.hi) rc = ss.upload(kAuxWrapHi, c.in, plane, &wrap[1]);
+      rc = ss.upload(kAuxPreA, t->pre_a, operand_span(t->pre_a_strides, c0.shape, ndim, es), &d_pre_a);
+    if (rc == XG_OK && wrap_lo)
+      rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c0.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
+    if (rc == XG_OK && wrap_hi) rc = ss.upload(kAuxWrapHi, c0.in, plane, &wrap[1]);
     if (rc == XG_OK) rc = ss.upload(kAuxFill, fill_host, es, &d_fill);
     if (rc == XG_OK) rc = ss.fence();
     if (rc) return rc;
 
-    PipeExtra ex;
-    if (ax0) {  // result rows [j0, j1) read planes [j0 - lo, j1 - lo] of the padded field
-      ex.lo_rows = lo;
-      ex.hi_rows = 1 - lo;
-      ex.edge_pairs = edge_pairs;
-    }
-    if (partner) {
-      ex.hin2 = partner;
-      ex.in2 = View3{1, n0, partner_row};
-    }
-    if (halo) ex.plane_row_bytes = (size_t)(vin.R / c.shape[c.axis]) * es;
-    int64_t sshape[XG_MAX_NDIM];
-    for (int d = 0; d < ndim; ++d) sshape[d] = c.shape[d];
     auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
-      sshape[0] = i1 - i0;
-      const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(i0 * c.pre_strides[0]) * es : nullptr;
-      const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * c.post_strides[0]) * es : nullptr;
-      // along dim 0 a slab pads only the edges of the field its planes reach
-      const int slo = ax0 ? j0 - lo < 0 : lo, shi = ax0 ? j1 - lo + 1 > n0 : c.hi;
-      const void* hl = slo ? wrap[0] : nullptr;
-      const void* hh = shi ? wrap[1] : nullptr;
-      if (halo) {
-        const int rc2 = halo(b, sshape, pm, d_fill, st, &hl, &hh);
+      for (int k = 0; k < nout; ++k) {
+        const Call& c = cs[k];
+        // the result's input rows [s0, s1); along dim 0 a slab pads only the edges of the field its rows reach
+        Window w{j0, j1, c.lo, c.hi};
+        if (c.axis == 0) {
+          const int rc2 = read_window(who, j0, j1, c.lo, n0, i0, i1, &w);
+          if (rc2) return rc2;
+        }
+        int64_t sshape[XG_MAX_NDIM];
+        for (int d = 0; d < ndim; ++d) sshape[d] = c.shape[d];
+        sshape[0] = w.s1 - w.s0;
+        const char* src = static_cast<const char*>(b.in) + (size_t)(w.s0 - i0) * plane;
+        const char* pm = d_pre ? static_cast<const char*>(d_pre) + (size_t)(w.s0 * c.pre_strides[0]) * es : nullptr;
+        const char* qm = d_post ? static_cast<const char*>(d_post) + (size_t)(j0 * c.post_strides[0]) * es : nullptr;
+        const bool wraps = c.axis == 0 && c.bc == XG_BC_PERIODIC;
+        const void* hl = wraps && w.slo ? wrap[0] : nullptr;
+        const void* hh = wraps && w.shi ? wrap[1] : nullptr;
+        if (halo) {
+          const int rc2 = halo(b, sshape, pm, d_fill, st, &hl, &hh);
+          if (rc2) return rc2;
+        }
+        const char* am =
+            d_pre_a ? static_cast<const char*>(d_pre_a) + (size_t)(w.s0 * t->pre_a_strides[0]) * es : nullptr;
+        const int rc2 =
+            t ? xg_stencil_pair_halo(c.dtype, src, b.in2, b.out[k], ndim, sshape, t->op_a, t->lo_a, t->hi_a, t->bc_a,
+                                     t->fill_a, am, t->pre_a_strides, c.axis, c.op, c.lo, c.hi, c.bc, c.fill_value,
+                                     pm, c.pre_strides, t->subtract, qm, c.post_strides, hl, hh, st)
+              : xg_stencil2(c.op, c.dtype, src, b.out[k], ndim, sshape, c.axis, w.slo, w.shi,
+                            (w.slo || w.shi) ? c.bc : XG_BC_NONE, c.fill_value, pm, c.pre_strides, qm, c.post_strides,
+                            hl, hh, st);
         if (rc2) return rc2;
       }
-      if (t) {
-        const char* am =
-            d_pre_a ? static_cast<const char*>(d_pre_a) + (size_t)(i0 * t->pre_a_strides[0]) * es : nullptr;
-        return xg_stencil_pair_halo(c.dtype, b.in, b.in2, b.out[0], ndim, sshape, t->op_a, t->lo_a, t->hi_a, t->bc_a,
-                                    t->fill_a, am, t->pre_a_strides, c.axis, c.op, lo, c.hi, c.bc, c.fill_value, pm,
-                                    c.pre_strides, t->subtract, qm, c.post_strides, hl, hh, st);
-      }
-      return xg_stencil2(c.op, c.dtype, b.in, b.out[0], ndim, sshape, c.axis, slo, shi,
-                         (slo || shi) ? c.bc : XG_BC_NONE, c.fill_value, pm, c.pre_strides, qm, c.post_strides, hl, hh,
-                         st);
+      return XG_OK;
     };
-    void* outs[1] = {c.out};
-    return ss.run(es, c.in, vin, 1, outs, &vout, launch, ex.rows(r0, r1));
+    void* outs[kMaxOut];
+    for (int k = 0; k < nout; ++k) outs[k] = cs[k].out;
+    return ss.run(es, c0.in, vin, nout, outs, vout, launch, ex.rows(r0, r1));
   });
 }
 
@@ -949,7 +985,44 @@ extern "C" int xg_stencil2_host(int op, int dtype, const void* in, void* out, in
   const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, bc, fill_value,
                pre_metric, pre_strides, post_metric, post_strides, device};
   int rc = validate_call("xg_stencil2_host", c);
-  return rc ? rc : stencil_host("xg_stencil2_host", c, nullptr, nullptr, 0, nullptr);
+  return rc ? rc : stencil_host("xg_stencil2_host", 1, &c, nullptr, nullptr, 0, nullptr);
+}
+
+extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const void* in, void* const* out, int ndim,
+                                      const int64_t* shape, const int* axis, const int* lo, const int* hi,
+                                      const int* bc, const double* fill_value, int device) {
+  const char* who = "xg_stencil2_host_multi";
+  const std::string w(who);
+  if (!in || !out || !shape || !op || !axis || !lo || !hi || !bc || !fill_value)
+    return xg_fail(XG_EINVAL, w + ": null pointer");
+  if (nout < 1 || nout > kMaxOut)
+    return xg_fail(XG_EINVAL, w + ": between 1 and " + std::to_string(kMaxOut) + " results per call");
+  Call cs[kMaxOut];
+  for (int k = 0; k < nout; ++k) {
+    if (!out[k]) return xg_fail(XG_EINVAL, w + ": null result pointer");
+    cs[k] = Call{op[k], dtype, in, out[k], ndim, shape, axis[k], lo[k], hi[k], bc[k], fill_value[k],
+                 nullptr, nullptr, nullptr, nullptr, device};
+    int rc = validate_call(who, cs[k]);
+    if (rc) return rc;
+    // slabs are cut along dim 0: a result operated along it must keep that extent (center <-> left / right shifts)
+    // and be padded at the field's ends only
+    if (axis[k] == 0 && lo[k] + hi[k] != 1)
+      return xg_fail(XG_ENOTIMPL, w + ": outer / inner shifts along the outermost dimension; use xg_stencil2_host "
+                                      "for that result");
+    if (axis[k] == 0 && bc[k] == XG_BC_EXTRAPOLATE)
+      return xg_fail(XG_ENOTIMPL, w + ": extrapolate along the outermost dimension");
+    // xg_stencil2 rejects an unknown code even where it pads nothing, and is given XG_BC_NONE there
+    if (bc[k] < XG_BC_NONE || bc[k] > XG_BC_EXTRAPOLATE)
+      return xg_fail(XG_EINVAL, "xg_stencil2: unknown boundary condition");
+  }
+  for (int k = 0; k < nout; ++k) {
+    int64_t out_shape[XG_MAX_NDIM];
+    for (int d = 0; d < ndim; ++d) out_shape[d] = shape[d];
+    out_shape[axis[k]] += lo[k] + hi[k] - 1;
+    const View3 v = view3(ndim, out_shape, 0);
+    if (v.L == 0 || v.R == 0) return xg_fail(XG_EINVAL, w + ": empty result");
+  }
+  return stencil_host(who, nout, cs, nullptr, nullptr, 0, nullptr);
 }
 
 extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
@@ -963,7 +1036,8 @@ extern "C" int xg_stencil2_host_fold(int op, int dtype, const void* in, void* ou
   int rc = validate_halo_call(who, c);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
   return rc ? rc
-            : stencil_host(who, c, nullptr, nullptr, 0, fold_stage(c, false, seam_axis, skip, mirror, period, negate));
+            : stencil_host(who, 1, &c, nullptr, nullptr, 0,
+                           fold_stage(c, false, seam_axis, skip, mirror, period, negate));
 }
 
 extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, const void* partner,
@@ -1001,7 +1075,7 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   const size_t es = dtype == XG_F32 ? 4 : 8;
   const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
   const void* fill_host = fill ? (es == 4 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
-  return stencil_host(who.c_str(), c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
+  return stencil_host(who.c_str(), 1, &c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
                       fill_host);
 }
 
@@ -1121,7 +1195,7 @@ extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, voi
   const Call c{op_b, dtype, a, out, ndim, shape, axis_b, lo_b, hi_b, bc_b, fill_b,
                pre_b, pre_b_strides, post, post_strides, device};
   int rc = validate_pair_call("xg_stencil_pair_host", c, t);
-  return rc ? rc : stencil_host("xg_stencil_pair_host", c, &t, b, view3(ndim, shape, 0).R, nullptr);
+  return rc ? rc : stencil_host("xg_stencil_pair_host", 1, &c, &t, b, view3(ndim, shape, 0).R, nullptr);
 }
 
 extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b, void* out, int ndim,
@@ -1138,6 +1212,6 @@ extern "C" int xg_stencil_pair_host_fold(int dtype, const void* a, const void* b
   int rc = validate_pair_call(who, c, t);
   if (rc == XG_OK) rc = validate_fold(who, c, seam_axis, skip, mirror, period);
   return rc ? rc
-            : stencil_host(who, c, &t, b, view3(ndim, shape, 0).R,
+            : stencil_host(who, 1, &c, &t, b, view3(ndim, shape, 0).R,
                            fold_stage(c, true, seam_axis, skip, mirror, period, negate));
 }

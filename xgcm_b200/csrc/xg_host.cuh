@@ -99,6 +99,16 @@ class Session {
   std::unique_lock<std::mutex> lock_;
 };
 
+// The input rows a slab of result rows [j0, j1) reads along the dim it is cut along, for a stencil of lower halo
+// width `lo` there on a field of extent n: rows [j0 - lo, j1 - lo + 1) clipped to [0, n) are [s0, s1), and slo / shi
+// tell whether they reach the field's lower / upper edge, the only ones the call's boundary condition pads.
+struct Window {
+  int64_t s0, s1;
+  int slo, shi;
+};
+// XG_EINVAL when the window leaves the slab's input rows [i0, i1)
+int read_window(const char* who, int64_t j0, int64_t j1, int lo, int64_t n, int64_t i0, int64_t i1, Window* w);
+
 // bytes spanned by a broadcast operand laid out with `strides` over `shape`
 size_t operand_span(const int64_t* strides, const int64_t* shape, int ndim, size_t es);
 

@@ -1,10 +1,7 @@
 // Host-buffer entry points beyond the stencils of xg_host.cu, on the same slab engine (xg_host.cuh), with
-// (a) several results per uploaded slab and (b) slabs cut along a dimension that is not the outermost one
-// (strided 2-D copies), so that every device entry point has a host twin:
+// slabs cut along a dimension that is not the outermost one (strided 2-D copies), so that every device entry point
+// has a host twin:
 //
-//   xg_stencil2_host_multi   one field up, K (op, axis, shift, boundary) results down: a `Grid.diff` +
-//                            `Grid.interp` sweep over X, Y, Z moves the field over PCIe once, not six
-//                            times (xgcm/grid.py:796-832 would re-read it per call).
 //   xg_stencil_multi_host    xgcm/grid.py:798-832 (a multi-axis diff / interp / min / max): one
 //                            xg_stencil_multi launch per slab
 //   xg_cumscan_host          xgcm/grid.py:1306-1414 on numpy-backed fields
@@ -17,12 +14,10 @@
 // contiguous elements -> one cudaMemcpy2DAsync each way.  Lines along the operated axis stay whole, so
 // no halo exchange between slabs is needed and summation order is untouched.  xg_cumscan_host and
 // xg_wreduce_host cut the first non-operated dim, and upload their metric / weight whole, once.
-// xg_stencil2_host_multi cuts dim 0; results operated along it read the rows around each slab, which the
-// engine carries over from the previous slab on the device.
 //
 // The two multi-axis twins cut the outermost dim of extent > 1 that is not operated, so every operated line is
 // whole in a slab.  When every dim of extent > 1 is operated, xg_stencil_multi_host cuts the outermost one and
-// reads the row next to each slab (as xg_stencil2_host_multi does along dim 0), and xg_wreduce_host_multi keeps
+// reads the row next to each slab (as the stencils of xg_host.cu do along dim 0), and xg_wreduce_host_multi keeps
 // one partial per index of it on the device and runs the launches along it once, at the end.
 //
 // The two transform twins pick the outermost non-operated dim of extent > 1 one index of which (its phi,
@@ -229,105 +224,6 @@ TransformViews transform_views(int ndim, const int64_t* shape, int axis, int64_t
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------
-extern "C" int xg_stencil2_host_multi(int nout, const int* op, int dtype, const void* in, void* const* out, int ndim,
-                                      const int64_t* shape, const int* axis, const int* lo, const int* hi,
-                                      const int* bc, const double* fill_value, int device) {
-  if (!in || !out || !shape || !op || !axis || !lo || !hi || !bc || !fill_value)
-    return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: null pointer");
-  if (nout < 1 || nout > kMaxOut)
-    return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: between 1 and " + std::to_string(kMaxOut) + " results per call");
-  if (dtype != XG_F32 && dtype != XG_F64)
-    return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: dtype must be XG_F32 or XG_F64");
-  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: bad ndim");
-  const size_t es = dtype == XG_F32 ? 4 : 8;
-  PipeExtra ex;  // each slab reads the rows around it that its results along dim 0 need
-  for (int k = 0; k < nout; ++k) {
-    if (!out[k]) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: null result pointer");
-    if (axis[k] < 0 || axis[k] >= ndim) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: axis out of range");
-    if (lo[k] < 0 || lo[k] > 1 || hi[k] < 0 || hi[k] > 1)
-      return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: halo widths must be 0 or 1");
-    if ((lo[k] || hi[k]) && (bc[k] <= XG_BC_NONE || bc[k] > XG_BC_EXTRAPOLATE))
-      return xg_fail(XG_EINVAL,
-                     "xg_stencil2_host_multi: no boundary condition was specified but the operation needs to "
-                     "pad the axis");
-    if (shape[axis[k]] == 0) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: empty operated axis");
-    if (axis[k] == 0) {
-      // slabs are cut along dim 0: a result operated along it must keep that extent (center <-> left / right
-      // shifts), and its halo must be expressible per slab
-      if (lo[k] + hi[k] != 1)
-        return xg_fail(XG_ENOTIMPL,
-                       "xg_stencil2_host_multi: outer / inner shifts along the outermost dimension; use "
-                       "xg_stencil2_host for that result");
-      if (bc[k] == XG_BC_EXTRAPOLATE)
-        return xg_fail(XG_ENOTIMPL, "xg_stencil2_host_multi: extrapolate along the outermost dimension");
-      if (lo[k] > ex.lo_rows) ex.lo_rows = lo[k];
-      if (hi[k] > ex.hi_rows) ex.hi_rows = hi[k];
-    }
-  }
-  // every result keeps the extent of dim 0, the slab dim
-  return spread("xg_stencil2_host_multi", device, shape[0], false, [&](int dev, int64_t r0, int64_t r1) -> int {
-    Session ss;
-    int rc = ss.open(dev);
-    if (rc) return rc;
-
-    const View3 vin = view3(ndim, shape, 0);
-    View3 vout[kMaxOut];
-    int64_t out_shape[kMaxOut][XG_MAX_NDIM];
-    for (int k = 0; k < nout; ++k) {
-      for (int d = 0; d < ndim; ++d) out_shape[k][d] = shape[d];
-      out_shape[k][axis[k]] = shape[axis[k]] + lo[k] + hi[k] - 1;
-      vout[k] = view3(ndim, out_shape[k], 0);
-      if (vout[k].R == 0 || vout[k].L == 0) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: empty result");
-    }
-    const int64_t n0 = shape[0];
-    // periodic wrap planes for results operated along dim 0: plane n0-1 below the first slab, plane 0 above the last
-    const void* d_wrap[2] = {nullptr, nullptr};
-    bool need_wrap = false;
-    for (int k = 0; k < nout; ++k) need_wrap = need_wrap || (axis[k] == 0 && bc[k] == XG_BC_PERIODIC);
-    if (need_wrap) {
-      const size_t pb = (size_t)vin.R * es;
-      rc = ss.upload(kAuxWrapLo, static_cast<const char*>(in) + (size_t)(n0 - 1) * pb, pb, &d_wrap[0]);
-      if (rc == XG_OK) rc = ss.upload(kAuxWrapHi, in, pb, &d_wrap[1]);
-      if (rc == XG_OK) rc = ss.fence();
-      if (rc) return rc;
-    }
-    auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
-      int64_t sshape[XG_MAX_NDIM];
-      for (int d = 0; d < ndim; ++d) sshape[d] = shape[d];
-      for (int k = 0; k < nout; ++k) {
-        const char* src = static_cast<const char*>(b.in);
-        int slo = lo[k], shi = hi[k], sbc = bc[k];
-        const void* hl = nullptr;
-        const void* hh = nullptr;
-        if (axis[k] == 0) {
-          // output rows [j0, j1) need P[j0 .. j1], i.e. source planes [j0 - lo, j1 - lo] clipped to the field
-          int64_t s0 = j0 - lo[k], s1 = j1 - lo[k] + 1;
-          slo = shi = 0;
-          if (s0 < 0) { s0 = 0; slo = 1; }
-          if (s1 > n0) { s1 = n0; shi = 1; }
-          if (s0 < i0 || s1 > i1) return xg_fail(XG_EINVAL, "xg_stencil2_host_multi: internal slab window error");
-          src += (size_t)(s0 - i0) * vin.R * es;
-          sshape[0] = s1 - s0;
-          if (bc[k] == XG_BC_PERIODIC) {
-            if (slo) hl = d_wrap[0];
-            if (shi) hh = d_wrap[1];
-          }
-          if (!slo && !shi) sbc = XG_BC_NONE;
-        } else {
-          src += (size_t)(j0 - i0) * vin.R * es;
-          sshape[0] = j1 - j0;
-        }
-        const int rc2 = xg_stencil2(op[k], dtype, src, b.out[k], ndim, sshape, axis[k], slo, shi, sbc, fill_value[k],
-                                    nullptr, nullptr, nullptr, nullptr, hl, hh, st);
-        if (rc2) return rc2;
-      }
-      return XG_OK;
-    };
-    return ss.run(es, in, vin, nout, out, vout, launch, ex.rows(r0, r1));
-  });
-}
-
-// ---------------------------------------------------------------------------------------------------
 extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
                                      const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
                                      const double* fill_value, int device) {
@@ -408,16 +304,16 @@ extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int n
       }
       const char* src = static_cast<const char*>(b.in);
       if (ka >= 0) {
-        // result rows [j0, j1) need padded planes [j0, j1], i.e. input rows [j0 - lo, j1 - lo] clipped to the field:
         // an inner slab edge reads its neighbour row, the field's own ends keep the call's boundary condition
-        int64_t s0 = j0 - lo[ka], s1 = j1 - lo[ka] + 1;
-        slo[ka] = shi[ka] = 0;
-        if (s0 < 0) { s0 = 0; slo[ka] = 1; }
-        if (s1 > n) { s1 = n; shi[ka] = 1; }
-        if (s0 < i0 || s1 > i1 || vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
-        if (!slo[ka] && !shi[ka]) sbc[ka] = XG_BC_NONE;
-        src += (size_t)(s0 - i0) * vin.R * es;
-        sshape[sd] = s1 - s0;
+        if (vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
+        Window w;
+        const int rc2 = read_window(who.c_str(), j0, j1, lo[ka], n, i0, i1, &w);
+        if (rc2) return rc2;
+        slo[ka] = w.slo;
+        shi[ka] = w.shi;
+        if (!w.slo && !w.shi) sbc[ka] = XG_BC_NONE;
+        src += (size_t)(w.s0 - i0) * vin.R * es;
+        sshape[sd] = w.s1 - w.s0;
       } else {
         sshape[sd] = j1 - j0;
       }
