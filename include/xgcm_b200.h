@@ -340,6 +340,15 @@ XG_API int xg_stencil2_host(int op, int dtype, const void* in, void* out, int nd
  * dim-0 strides of the plane and of its source (0 for the constant).  The copies must write disjoint
  * cells that cover each padded plane.  `partner` (optional, shape `partner_shape`, same ndim and dim-0
  * extent as the field) is streamed slab by slab beside it.  No pre-metric.
+ *
+ * _connected_weighted: _connected with a pre-metric (`pre_metric` / `pre_strides` as in _fold, uploaded whole)
+ * and no partner (source 1 is XG_EINVAL).  The stencil reads x * pre, rounded once in the field's dtype: the kernel
+ * forms it inside the slab, and the halo planes hold the gathered x times the gathered metric.  Copy k also reads
+ * the metric cells at element offset pre_offset[k] with strides pre_src_strides[k * copy_ndim ..] (0 where the
+ * metric broadcasts; dim-0 stride that of pre_strides), or, for a fill copy, the constant 1 (offset 0, strides 0),
+ * so a fill edge stays the bare fill value.  Per slab, one xg_strided_copy_batch launch writes the planes and the
+ * weight planes (workspace scratch, two planes per slab row), one xg_binary launch per padded plane multiplies
+ * them, then the xg_stencil2 launch takes the pre- and post-metric and the planes.
  */
 XG_API int xg_stencil2_host_fold(int op, int dtype, const void* in, void* out, int ndim,
                                  const int64_t* shape, int axis, int lo, int hi, int bc,
@@ -354,6 +363,15 @@ XG_API int xg_stencil2_host_connected(int op, int dtype, const void* in, const v
                                       const int64_t* dst_offset, const int64_t* src_offset,
                                       const int64_t* shapes, const int64_t* dst_strides,
                                       const int64_t* src_strides, const int* negate, int device);
+XG_API int xg_stencil2_host_connected_weighted(int op, int dtype, const void* in, void* out, int ndim,
+                                               const int64_t* shape, int axis, int lo, int hi, double fill_value,
+                                               const void* pre_metric, const int64_t* pre_strides,
+                                               const void* post_metric, const int64_t* post_strides, int ncopies,
+                                               int copy_ndim, const int* side, const int* source,
+                                               const int64_t* dst_offset, const int64_t* src_offset,
+                                               const int64_t* pre_offset, const int64_t* shapes,
+                                               const int64_t* dst_strides, const int64_t* src_strides,
+                                               const int64_t* pre_src_strides, const int* negate, int device);
 
 /*
  * A multi-axis diff / interp / min / max of a HOST field on the two grid topologies whose halo is not a boundary

@@ -99,6 +99,11 @@ SIGNATURES = {
         [C.c_int, C.c_int, _vp, _vp, _i64p, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_double,
          _vp, _i64p, C.c_int, C.c_int, _i32p, _i32p, _i64p, _i64p, _i64p, _i64p, _i64p, _i32p, C.c_int],
     ),
+    "xg_stencil2_host_connected_weighted": (
+        C.c_int,
+        [C.c_int, C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_double, _vp, _i64p, _vp, _i64p,
+         C.c_int, C.c_int, _i32p, _i32p, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _i64p, _i32p, C.c_int],
+    ),
     "xg_stencil_chain_host_fold": (
         C.c_int,
         [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, _i32p, _i32p, _i32p, _i32p, _i32p, _f64p, _i32p, _i32p, _i32p,

@@ -24,7 +24,8 @@
 // xg_stencil2_host_fold / xg_stencil2_host_connected: dim 0 is a batch dim, and a per-slab halo stage on the kernel
 // stream builds the slab's halo_lo / halo_hi planes from the slab buffers (one xg_fold_rows launch, or the
 // face-connection copy list clipped to the slab and replayed with xg_strided_copy_batch) just before its
-// xg_stencil2 launch.  xg_stencil_pair_host / xg_stencil_pair_host_fold: field a is the slab input, field b the
+// xg_stencil2 launch; xg_stencil2_host_connected_weighted replays the copy list over the pre-metric too and multiplies
+// the planes by those weights (xg_binary), the halo of x * pre.  xg_stencil_pair_host / xg_stencil_pair_host_fold: field a is the slab input, field b the
 // second streamed input, and each slab is one xg_stencil_pair_halo launch (after the xg_fold_rows launch of b's
 // folded row, for the fold).  xg_cumscan_host_fold / xg_cumscan_host_connected run the same halo stages on each
 // slab's scanned rows (xg_cumscan into the scratch buffer), then place the scanned slab and its halo planes into the
@@ -511,8 +512,10 @@ HaloFn fold_stage(const Call& c, bool of_in2, int seam_axis, int skip, int64_t m
 // (field b of pair `t`, or the partner vector component, `partner_row` elements per dim-0 index) beside the field,
 // the metrics (and the `fill_host` constant, es bytes, when given) uploaded whole, and per slab `halo` (when dim 0 is
 // a batch dim) building the halo planes.  Per slab, one xg_stencil2 or xg_stencil_pair_halo launch per result.
+// `fill_host` holds `nfill` constants; `scratch_row_bytes` sizes the scratch buffer per slab row (halo stages only).
 int stencil_host(const char* who, int nout, const Call* cs, const PairTerm* t, const void* partner,
-                 int64_t partner_row, const HaloFn& halo, const void* fill_host = nullptr) {
+                 int64_t partner_row, const HaloFn& halo, const void* fill_host = nullptr, int nfill = 1,
+                 size_t scratch_row_bytes = 0) {
   const Call& c0 = cs[0];
   const size_t es = c0.dtype == XG_F32 ? 4 : 8;
   const int ndim = c0.ndim;
@@ -540,7 +543,10 @@ int stencil_host(const char* who, int nout, const Call* cs, const PairTerm* t, c
     ex.hin2 = partner;
     ex.in2 = View3{1, n0, partner_row};
   }
-  if (halo) ex.plane_row_bytes = (size_t)(vin.R / c0.shape[c0.axis]) * es;
+  if (halo) {
+    ex.plane_row_bytes = (size_t)(vin.R / c0.shape[c0.axis]) * es;
+    ex.scratch_row_bytes = scratch_row_bytes;
+  }
   return spread(who, c0.device, vout[0].L, ex.edge_pairs, [&](int device, int64_t r0, int64_t r1) -> int {
     Session ss;
     int rc = ss.open(device);
@@ -558,7 +564,7 @@ int stencil_host(const char* who, int nout, const Call* cs, const PairTerm* t, c
     if (rc == XG_OK && wrap_lo)
       rc = ss.upload(kAuxWrapLo, static_cast<const char*>(c0.in) + (size_t)(n0 - 1) * plane, plane, &wrap[0]);
     if (rc == XG_OK && wrap_hi) rc = ss.upload(kAuxWrapHi, c0.in, plane, &wrap[1]);
-    if (rc == XG_OK) rc = ss.upload(kAuxFill, fill_host, es, &d_fill);
+    if (rc == XG_OK) rc = ss.upload(kAuxFill, fill_host, (size_t)nfill * es, &d_fill);
     if (rc == XG_OK) rc = ss.fence();
     if (rc) return rc;
 
@@ -702,6 +708,61 @@ HaloFn copy_stage(const CopyList& cl, int dtype, int lo, int hi) {
                             cl.negate[k], st);
       if (rc2) return rc2;
     }
+    return XG_OK;
+  };
+}
+
+// The weighted face connections' halo stage: the halo of x * pre.  One xg_strided_copy_batch launch runs the copy
+// list twice: over the field into the halo planes, and over the slab's rows of the pre-metric (copy k reads it at
+// pre_offset[k] with pre_src_strides[k]; a fill copy reads the constant 1 after the fill value) into two weight planes
+// in the scratch buffer.  One xg_binary launch per padded plane then multiplies it by its weight plane in place, so
+// each halo cell is the gathered x times the gathered metric, rounded once, and a fill edge stays the fill value.
+HaloFn weighted_copy_stage(const CopyList& cl, const int64_t* pre_offset, const int64_t* pre_src_strides, int dtype,
+                           int axis, int ndim, int lo, int hi) {
+  return [=](const SlabBufs& b, const int64_t* slab_shape, const void* pre, const void* d_fill, cudaStream_t st,
+             const void** hl, const void** hh) -> int {
+    const size_t es = dtype == XG_F32 ? 4 : 8;
+    int64_t plane_elems = 1;
+    for (int d = 0; d < ndim; ++d)
+      if (d != axis) plane_elems *= slab_shape[d];
+    void* weight[2] = {b.scratch, static_cast<char*>(b.scratch) + (size_t)plane_elems * es};
+    const size_t n = (size_t)cl.n, nd = (size_t)cl.ndim;
+    std::vector<void*> dptr(2 * n);
+    std::vector<const void*> sptr(2 * n);
+    std::vector<int64_t> shp(2 * n * nd), dstr(2 * n * nd), sstr(2 * n * nd);
+    std::vector<int> neg(2 * n, 0);
+    for (size_t k = 0; k < n; ++k) {
+      const bool from_fill = cl.source[k] == kSrcFill;
+      dptr[k] = static_cast<char*>(b.plane[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
+      sptr[k] = static_cast<const char*>(from_fill ? d_fill : b.in) + (size_t)cl.src_offset[k] * es;
+      dptr[n + k] = static_cast<char*>(weight[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
+      sptr[n + k] = from_fill ? static_cast<const char*>(d_fill) + es
+                              : static_cast<const char*>(pre) + (size_t)pre_offset[k] * es;
+      for (size_t d = 0; d < nd; ++d) {
+        shp[k * nd + d] = shp[(n + k) * nd + d] = d ? cl.shapes[k * nd + d] : slab_shape[0];
+        dstr[k * nd + d] = dstr[(n + k) * nd + d] = cl.dst_strides[k * nd + d];
+        sstr[k * nd + d] = cl.src_strides[k * nd + d];
+        sstr[(n + k) * nd + d] = pre_src_strides[k * nd + d];
+      }
+      neg[k] = cl.negate[k];
+    }
+    int rc2 = xg_strided_copy_batch(dtype, (int)(2 * n), dptr.data(), sptr.data(), cl.ndim, shp.data(), dstr.data(),
+                                    sstr.data(), neg.data(), st);
+    if (rc2 == XG_ENOTIMPL) {  // some copy does not collapse to 5 dims: one launch per copy
+      rc2 = XG_OK;
+      for (size_t k = 0; rc2 == XG_OK && k < 2 * n; ++k)
+        rc2 = xg_strided_copy(dtype, dptr[k], dstr.data() + k * nd, sptr[k], sstr.data() + k * nd, cl.ndim,
+                              shp.data() + k * nd, neg[k], st);
+    }
+    if (rc2) return rc2;
+    const int64_t unit = 1;
+    for (int side = 0; side < 2; ++side) {
+      if (!(side ? hi : lo)) continue;
+      rc2 = xg_binary(XG_BIN_MUL, dtype, b.plane[side], weight[side], &unit, b.plane[side], 1, &plane_elems, st);
+      if (rc2) return rc2;
+    }
+    if (lo) *hl = b.plane[0];
+    if (hi) *hh = b.plane[1];
     return XG_OK;
   };
 }
@@ -1077,6 +1138,57 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   const void* fill_host = fill ? (es == 4 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
   return stencil_host(who.c_str(), 1, &c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
                       fill_host);
+}
+
+extern "C" int xg_stencil2_host_connected_weighted(
+    int op, int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis, int lo, int hi,
+    double fill_value, const void* pre_metric, const int64_t* pre_strides, const void* post_metric,
+    const int64_t* post_strides, int ncopies, int copy_ndim, const int* side, const int* source,
+    const int64_t* dst_offset, const int64_t* src_offset, const int64_t* pre_offset, const int64_t* shapes,
+    const int64_t* dst_strides, const int64_t* src_strides, const int64_t* pre_src_strides, const int* negate,
+    int device) {
+  const std::string who = "xg_stencil2_host_connected_weighted";
+  const Call c{op, dtype, in, out, ndim, shape, axis, lo, hi, (lo || hi) ? XG_BC_FILL : XG_BC_NONE,
+               fill_value, pre_metric, pre_strides, post_metric, post_strides, device};
+  const CopyList cl{ncopies, copy_ndim, side, source, dst_offset, src_offset, shapes, dst_strides, src_strides, negate};
+  int rc = validate_halo_call(who.c_str(), c);
+  if (rc) return rc;
+  if (!pre_metric || !pre_strides) return xg_fail(XG_EINVAL, who + ": null pre-metric");
+  const int64_t n0 = shape[0];
+  int64_t row_in = 1;
+  for (int d = 1; d < ndim; ++d) row_in *= shape[d];
+  const int64_t plane_row = shape[axis] ? row_in / shape[axis] : 0;
+  bool fill = false;
+  rc = validate_copies(who, cl, lo, hi, n0, plane_row, row_in, false, 0, &fill);
+  if (rc) return rc;
+  if (ncopies > 0 && (!pre_offset || !pre_src_strides)) return xg_fail(XG_EINVAL, who + ": null pointer in the copy list");
+  // the metric copies: inside the pre-metric, with its dim-0 stride, or the constant 1 at offset 0, strides 0
+  const size_t es = dtype == XG_F32 ? 4 : 8;
+  const int64_t pre_elems = (int64_t)(operand_span(pre_strides, shape, ndim, es) / es);
+  for (int k = 0; k < ncopies; ++k) {
+    const int64_t* ps = pre_src_strides + (size_t)k * copy_ndim;
+    const std::string at = who + ": copy " + std::to_string(k) + ": ";
+    if (ps[0] != (source[k] == kSrcFill ? 0 : pre_strides[0]))
+      return xg_fail(XG_EINVAL, at + "the pre-metric copy must span dim 0 with the pre-metric's dim-0 stride");
+    const int64_t* sh = shapes + (size_t)k * copy_ndim;
+    int64_t cells = 1;
+    for (int d = 0; d < copy_ndim; ++d) cells *= sh[d];
+    if (cells == 0) continue;
+    int64_t a, b;
+    copy_extent(pre_offset[k], ps, sh, copy_ndim, &a, &b);
+    if (source[k] == kSrcFill) {
+      if (a != 0 || b != 0) return xg_fail(XG_EINVAL, at + "the constant 1 is read with offset 0, strides 0");
+    } else if (a < 0 || b >= pre_elems) {
+      return xg_fail(XG_EINVAL, at + "leaves the pre-metric");
+    }
+  }
+  // the fill value, then the weight of a fill edge (1)
+  const float f32[2] = {(float)fill_value, 1.0f};  // pageable: staged before cudaMemcpyAsync returns
+  const double f64[2] = {fill_value, 1.0};
+  const void* fill_host = fill ? (es == 4 ? (const void*)f32 : (const void*)f64) : nullptr;
+  return stencil_host(who.c_str(), 1, &c, nullptr, nullptr, 0,
+                      weighted_copy_stage(cl, pre_offset, pre_src_strides, dtype, axis, ndim, lo, hi), fill_host, 2,
+                      2 * (size_t)plane_row * es);
 }
 
 extern "C" int xg_cumscan_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,

@@ -1088,9 +1088,9 @@ class Grid:
         ``_connected`` where the padded edge crosses a north fold or a face connection.  Those two run per slab
         the device route's scan, halo of the scanned field (as ``pad`` builds it) and divide by the post metric;
         their slabs are cut as the stencils cut them (``grid_ufunc._host_stream_route``) and the halo is planned
-        for the scanned, merged layout.  Returns the result, or None: the whole-field route (a fold or connected
-        call with both cumint and metric_weighted, a per-side padding mapping, no batch dim in front of the halo
-        dims, a fold the plan cannot mirror)."""
+        for the scanned, merged layout.  Returns the result, or None: the whole-field route (a call with both
+        cumint and metric_weighted, a per-side padding mapping, no batch dim in front of the halo dims, a fold the
+        plan cannot mirror)."""
         from . import ops
         from .padding import _axis_dim, _fold_plan, connected_halo_program
 
@@ -1119,7 +1119,7 @@ class Grid:
             post = self._metric_host(self.get_metric(probe, s.weighted), out_dims, x.dtype)
         if pre_weight is not None:  # cumint: the metric product rides on the kernel's pre operand
             if pre is not None:
-                raise NotImplementedError("cumint with metric_weighted on a host array: pass a device array")
+                return None  # cumint with metric_weighted: two pre weights, the whole-field route
             pre = self._metric_host(pre_weight, dims, x.dtype)
         device = self._host_device(da)
         if halo is None:

@@ -541,24 +541,36 @@ def apply_as_grid_ufunc(
 def _apply_connected_stencil(op, da, raw_arg, other_component, grid, ax_name, in_dim, out_dim,
                              padding_width_real, padding, fill_value, pre_metric, post_metric_fn):
     """Built-in operator on a grid with face connections: the halo is not an affine function of
-    the field any more (it comes from other faces, rotated), so it is materialised once by
-    ``pad`` -> ``xg_strided_copy`` and the stencil then runs on the padded array without a
-    boundary condition (reference: grid_ufunc.py:903-921 pads, then applies the kernel)."""
+    the field any more (it comes from other faces, rotated).  A one-cell halo is gathered into thin
+    planes (``connected_halo_planes``, of ``x * pre`` under a pre-metric) that the fused stencil takes
+    beside the field; a numpy field streams in slabs that do the same.  A wider halo (user ufuncs) is
+    materialised by ``pad`` and the stencil runs on the padded array without a boundary condition
+    (reference: grid_ufunc.py:903-921 pads, then applies the kernel)."""
     from . import ops
     from .device import as_device_tensor, result_like
     from .padding import pad
 
     lo, hi = padding_width_real.get(ax_name, (0, 0))
-    if pre_metric is None and lo <= 1 and hi <= 1:
+    if pre_metric is not None and isinstance(raw_arg, dict):
+        raise NotImplementedError(
+            "metric weighting of vector components across face connections is not implemented"
+        )
+    if lo <= 1 and hi <= 1:
         streamed = _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi,
-                                             padding, fill_value, post_metric_fn)
+                                             padding, fill_value, post_metric_fn, pre_metric)
         if streamed is not None:
             return streamed
-        # halo planes gathered from the neighbour faces, then the ordinary fused launch
+        # halo planes gathered from the neighbour faces (of x * pre), then the ordinary fused launch
         from .padding import connected_halo_planes
 
-        x, halo_lo, halo_hi, was_host, dims = connected_halo_planes(
-            raw_arg, grid, ax_name, lo, hi, padding, fill_value, other_component)
+        arg, pre_t, was_host = raw_arg, None, None
+        if pre_metric is not None:
+            x, was_host = as_device_tensor(da.data, grid._device_for(da))
+            pre_t = grid._metric_tensor(pre_metric, da.dims, x)
+            arg = DataArray(x, dims=da.dims, name=da.name, attrs=da.attrs)
+        x, halo_lo, halo_hi, on_host, dims = connected_halo_planes(
+            arg, grid, ax_name, lo, hi, padding, fill_value, other_component, pre=pre_t)
+        was_host = on_host if was_host is None else was_host
         axis_num = dims.index(in_dim)
         out_dims = tuple(out_dim if d == in_dim else d for d in dims)
         out_shape = list(x.shape)
@@ -566,17 +578,12 @@ def _apply_connected_stencil(op, da, raw_arg, other_component, grid, ax_name, in
         post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
         post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
         out = ops.stencil2(x, axis_num, op, lo, hi, "fill" if (lo or hi) else None, 0.0,
-                           post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
+                           pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
         return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
     if pre_metric is not None:
-        if isinstance(raw_arg, dict):
-            raise NotImplementedError(
-                "metric weighting of vector components across face connections is not implemented"
-            )
-        x, was_host = as_device_tensor(da.data, grid._device_for(da))
-        x = ops.binary("mul", x, grid._metric_tensor(pre_metric, da.dims, x))
-        weighted = DataArray(result_like(x, was_host), dims=da.dims, name=da.name, attrs=da.attrs)
-        raw_arg = weighted
+        raise NotImplementedError(
+            "metric weighting across face connections takes a halo of at most one cell per side"
+        )
     padded = pad(raw_arg, grid=grid, padding_width={ax_name: (lo, hi)}, padding=padding,
                  fill_value=fill_value, other_component=other_component)
     if isinstance(padded, dict):  # zero-width request: pad returns its input untouched
@@ -735,11 +742,12 @@ def _merge_leading(a, ndrop, nmerge):
 
 
 def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi, padding,
-                              fill_value, post_metric_fn):
+                              fill_value, post_metric_fn, pre_metric=None):
     """A built-in operator on a numpy field of a grid with face connections through the host slab pipeline
-    (``xg_stencil2_host_connected``), or None when the field does not stream (``_host_stream_route``)."""
+    (``xg_stencil2_host_connected``, or ``xg_stencil2_host_connected_weighted`` with a ``pre_metric`` on a scalar
+    field), or None when the field does not stream (``_host_stream_route``)."""
     from . import ops
-    from .padding import (_axis_dim, _get_all_connection_axes, _unpack_vector, connected_edge_mode,
+    from .padding import (_get_all_connection_axes, _unpack_vector, broadcast_strides, connected_edge_mode,
                           connected_halo_program)
 
     da, isvector, vectoraxis, partner = _unpack_vector(grid, raw_arg, other_component)
@@ -757,23 +765,30 @@ def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_di
     out_shape[axis_num] = shape[axis_num] + lo + hi - 1
     post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
     post_h = None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype)
+    pre_h = None if pre_metric is None else grid._metric_host(pre_metric, dims, da.data.dtype)
     first = min(dims.index(d) for d in core)
     partner_ok = not isvector or (
         not partner.is_device and isinstance(partner.data, np.ndarray) and len(partner.dims) == len(dims)
         and tuple(partner.dims[:first]) == dims[:first] and tuple(partner.shape[:first]) == tuple(shape[:first]))
     cut = _host_stream_route("connected", dims, shape, core, lo, hi, partner_ok=partner_ok,
-                             operand_shapes=[post_h.shape] if post_h is not None else [])
+                             operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
     if cut is None:
         return None
-    m_dims = cut.dims(dims)
+    m_dims, m_shape = cut.dims(dims), cut.shape(shape)
+    kw = dict(post=cut.cut(post_h), device=grid._host_device(da))
+    if pre_h is not None:  # a scalar field (vector components with a pre-metric raise before this)
+        pre_m = cut.cut(pre_h)
+        program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode,
+                                         pre_strides=broadcast_strides(pre_m.shape, m_shape))
+        out = ops.stencil2_host_connected_weighted(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program,
+                                                   pre=pre_m, **kw)
+        return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
     q = partner_layout = None
     if isvector:
         q = cut.cut(partner.data)
         partner_layout = (cut.dims(partner.dims), tuple(q.shape))
-    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, cut.shape(shape), mode, vectoraxis,
-                                     partner_layout)
-    out = ops.stencil2_host_connected(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program, partner=q,
-                                      post=cut.cut(post_h), device=grid._host_device(da))
+    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode, vectoraxis, partner_layout)
+    out = ops.stencil2_host_connected(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program, partner=q, **kw)
     return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
 
 

@@ -715,6 +715,33 @@ def stencil2_host_connected(x: np.ndarray, axis: int, op: str, lo: int, hi: int,
     return out
 
 
+def stencil2_host_connected_weighted(x: np.ndarray, axis: int, op: str, lo: int, hi: int, fill_value: float,
+                                     program: Sequence[tuple], pre: np.ndarray, post: Optional[np.ndarray] = None,
+                                     out: Optional[np.ndarray] = None, device: HostDevice = None) -> np.ndarray:
+    """:func:`stencil2_host_connected` of ``x * pre`` (``xg_stencil2_host_connected_weighted``), divided by ``post``:
+    the metric-weighted operator of a scalar field across face connections.  ``program`` is the copy list of
+    ``padding.connected_halo_program`` with a metric layout, whose copies also carry the offset and strides of the
+    ``pre`` cells they read (the pre-metric broadcast against ``x``, strides 0 where it broadcasts); no partner."""
+    lib = _capi.load()
+    x, shape, axis, out, pre_op, post_op, dev = _host_stencil_prep(
+        x, axis, op, lo, hi, "fill" if (lo or hi) else None, pre, post, out, device,
+        "stencil2_host_connected_weighted")
+    if pre_op[0] is None:
+        raise ValueError("stencil2_host_connected_weighted: a pre-metric is required")
+    if any(len(c) != 10 or len(c[9]) != len(c[6]) for c in program):
+        raise ValueError("stencil2_host_connected_weighted: every copy must carry the metric offset and strides")
+    n, cndim, side, source, doff, soff, shapes, dstr, sstr, neg = _copy_list_args(program)
+    poff = _capi.i64_array([int(c[8]) for c in program] or [0])
+    pstr = _capi.i64_array([int(v) for c in program for v in c[9]] or [0])
+    rc = lib.xg_stencil2_host_connected_weighted(
+        _capi.OPS[op], _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape),
+        axis, lo, hi, float(fill_value), pre_op[1], pre_op[2], post_op[1], post_op[2], n, cndim, side, source, doff,
+        soff, poff, shapes, dstr, sstr, pstr, neg, dev,
+    )
+    _capi.check(rc)
+    return out
+
+
 def _chain_args(x, specs):
     """C-ABI values of the stages ``specs`` of a host chain (``_stencil_specs``): the count, the page-locked result,
     the int arrays of axes, op codes, lo and hi, the boundary codes, and the fills."""

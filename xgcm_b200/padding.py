@@ -297,6 +297,13 @@ def _contiguous_strides(shape):
     return list(reversed(strides))
 
 
+def broadcast_strides(m_shape, shape):
+    """Element strides of a C-contiguous operand of shape ``m_shape`` (1 where it broadcasts) read over ``shape``:
+    0 along every dim of extent 1 in either, as the kernels' operands take them."""
+    m_strides = _contiguous_strides(m_shape)
+    return [0 if int(m) == 1 or int(n) == 1 else st for m, n, st in zip(m_shape, shape, m_strides)]
+
+
 def _axis_dim(grid, dims, axname):
     for d in grid.axes[axname].coords.values():
         if d in dims:
@@ -489,7 +496,7 @@ def connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face
 
 
 def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout, face_offset=0,
-                        remote_edges=None):
+                        remote_edges=None, self_strides=None):
     """The strided copies that write the neighbour rims of every connected edge into the one-cell halo
     planes of a field with ``dims`` / ``shape`` along ``ax_name``: a list of ``(side, dst offset, dst strides,
     source ("self" or "partner"), src offset, src strides, shape, negate)``, offsets and strides in elements
@@ -498,16 +505,19 @@ def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner
 
     The index maps depend only on the topology and the array layout, not on the values: they are derived
     once per (axis, widths, layout) and kept on the grid.  ``face_offset`` / ``remote_edges`` as in
-    :func:`connected_halo_planes` (such plans are not cached)."""
+    :func:`connected_halo_planes` (such plans are not cached).  ``self_strides``: element strides "self" is read
+    with instead of the contiguous ones of ``shape`` -- a metric broadcast against the field, 0 where it
+    broadcasts, whose plan replays the field's index maps over the metric's cells."""
     facedim = grid._facedim
     face_links = grid._face_connections[facedim]
     isvector = partner_layout is not None
     cache = grid.__dict__.setdefault("_halo_plan_cache", {})
-    key = (ax_name, lo, hi, tuple(dims), tuple(shape), vectoraxis, partner_layout)
+    self_strides = _contiguous_strides(shape) if self_strides is None else [int(v) for v in self_strides]
+    key = (ax_name, lo, hi, tuple(dims), tuple(shape), vectoraxis, partner_layout, tuple(self_strides))
     plan = cache.get(key) if remote_edges is None else None
     if plan is not None:
         return plan
-    sources = {"self": ("self", tuple(dims), list(shape), _contiguous_strides(shape))}
+    sources = {"self": ("self", tuple(dims), list(shape), self_strides)}
     if isvector:
         p_dims, p_shape = partner_layout
         sources["partner"] = ("partner", tuple(p_dims), list(p_shape), _contiguous_strides(p_shape))
@@ -535,12 +545,18 @@ def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner
     return plan
 
 
-def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=None, partner_layout=None):
+def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=None, partner_layout=None,
+                           pre_strides=None):
     """Every strided copy that builds the one-cell halo planes of a field with ``dims`` / ``shape`` along
     ``ax_name``, for the host slab pipeline (``xg_stencil2_host_connected``), which replays the list on each
     slab: the neighbour rims of :func:`_connected_edge_plan` plus, on each face without a connection on a
     padded side, the basic boundary value (``mode``: fill from the constant, source ``"fill"``; extend: the
-    nearest row; periodic: the row at the other end).  Each face's plane is written by exactly one copy."""
+    nearest row; periodic: the row at the other end).  Each face's plane is written by exactly one copy.
+
+    ``pre_strides``: the element strides of a pre-metric read over ``shape`` (:func:`broadcast_strides`).  Each
+    copy then also carries ``(pre offset, pre strides)``, the metric cells under the field cells it reads (the
+    same index map over the metric; offset 0, strides 0 for a fill copy, whose weight is 1), for
+    ``xg_stencil2_host_connected_weighted``: the halo of ``x * pre``."""
     facedim = grid._facedim
     face_links = grid._face_connections[facedim]
     dims = tuple(dims)
@@ -553,6 +569,11 @@ def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=
     p_strides = _contiguous_strides(p_shape)
     loop = [d for d in range(len(dims)) if d != f]
     program = list(_connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout))
+    if pre_strides is not None:
+        ms = [int(v) for v in pre_strides]
+        weights = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout,
+                                       self_strides=ms)
+        program = [c + (w[4], w[5]) for c, w in zip(program, weights)]
     for side, w in ((0, lo), (1, hi)):
         if not w:
             continue
@@ -562,16 +583,19 @@ def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=
             c_shape = [p_shape[d] for d in loop]
             dst = (side, i * p_strides[f], [p_strides[d] for d in loop])
             if mode == "fill":
-                program.append(dst + ("fill", 0, [0] * len(loop), c_shape, False))
+                copy = dst + ("fill", 0, [0] * len(loop), c_shape, False)
+                weight = (0, [0] * len(loop))
             else:
                 row = ((n - 1) if side else 0) if mode == "extend" else (0 if side else (n - 1))
-                program.append(dst + ("self", i * strides[f] + row * strides[t], [strides[d] for d in loop],
-                                      c_shape, False))
+                copy = dst + ("self", i * strides[f] + row * strides[t], [strides[d] for d in loop], c_shape, False)
+                if pre_strides is not None:
+                    weight = (i * ms[f] + row * ms[t], [ms[d] for d in loop])
+            program.append(copy if pre_strides is None else copy + weight)
     return program
 
 
 def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_component=None,
-                          face_offset=0, remote_edges=None):
+                          face_offset=0, remote_edges=None, pre=None):
     """The one-cell halo planes of ``da`` along ``ax_name`` on a grid with face connections, for
     the fused stencil kernel (``xg_stencil2`` takes them as ``halo_lo`` / ``halo_hi``).
 
@@ -585,6 +609,12 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
     global face ``face_offset`` (faces sharded across GPUs, ``parallel.sharded_connected_stencil2``);
     edges whose neighbour lives in another block are not filled here but appended to
     ``remote_edges`` as ``(side, local face, connection)``.
+
+    ``pre`` (a device tensor that broadcasts against the scalar field, 1 where it broadcasts): the planes are
+    those of ``x * pre``, the halo of a metric-weighted operator, whose fused stencil then takes ``pre`` for the
+    interior cells.  The same copies run over the metric into weight planes (1 on a fill edge, which stays the
+    bare fill value, as the reference pads the already weighted array); one ``xg_binary`` launch multiplies the
+    two, so each halo cell is the gathered ``x`` times the gathered metric, rounded once in the field's dtype.
     """
     import torch
 
@@ -609,23 +639,38 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
     n = shape[t]
     n_face = shape[dims.index(facedim)]
     mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face_offset)
+    p_shape = list(shape)
+    p_shape[t] = 1
+    if pre is not None:
+        if isvector:
+            raise NotImplementedError(
+                "metric weighting of vector components across face connections is not implemented")
+        m = pre.to(x.dtype).contiguous()
+        m_strides = broadcast_strides(list(m.shape), shape)
+        # the x planes and the weight planes side by side: one product over both at the end
+        sides = [side for side, w in ((0, lo), (1, hi)) if w]
+        stack = torch.empty([2 * len(sides)] + p_shape, dtype=x.dtype, device=x.device)
+        weights = {side: stack[len(sides) + k] for k, side in enumerate(sides)}
     planes = []
     for side, w in ((0, lo), (1, hi)):
         if not w:
             planes.append(None)
             continue
-        p_shape = list(shape)
-        p_shape[t] = 1
+        plane = torch.empty(p_shape, dtype=x.dtype, device=x.device) if pre is None else stack[sides.index(side)]
         if mode == "fill":
-            plane = torch.full(p_shape, float(fv), dtype=x.dtype, device=x.device)
+            plane.fill_(float(fv))
+            if pre is not None:
+                weights[side].fill_(1.0)
         else:  # extend: nearest cell; periodic: the cell at the other end
-            plane = torch.empty(p_shape, dtype=x.dtype, device=x.device)
             if mode == "extend":
                 row = (n - 1) if side else 0
             else:
                 assert mode == "periodic"
                 row = 0 if side else (n - 1)
             ops.strided_copy(plane, 0, _contiguous_strides(p_shape), x, row * strides[t], strides, p_shape)
+            if pre is not None:
+                ops.strided_copy(weights[side], 0, _contiguous_strides(p_shape), m, row * m_strides[t], m_strides,
+                                 p_shape)
         planes.append(plane)
 
     partner_layout = None if not isvector else (sources["partner"][1], tuple(sources["partner"][2]))
@@ -633,7 +678,16 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
                                 face_offset, remote_edges)
     batch = [(planes[side], doff, dstr, sources[src_key][0], soff, sstr, shp, neg)
              for side, doff, dstr, src_key, soff, sstr, shp, neg in plan]
-    ops.strided_copy_batch(batch)  # both planes, every connected face: one launch
+    if pre is not None:  # the same index maps over the metric's cells
+        m_plan = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, None, None, face_offset,
+                                      [] if remote_edges is not None else None, self_strides=m_strides)
+        batch += [(weights[side], doff, dstr, m, soff, sstr, shp, False)
+                  for side, doff, dstr, _, soff, sstr, shp, _ in m_plan]
+    ops.strided_copy_batch(batch)  # both planes, every connected face (and their weights): one launch
+    if pre is not None and sides:
+        n_sides = len(sides)
+        weighted = ops.binary("mul", stack[:n_sides], stack[n_sides:])
+        planes = [None if not w else weighted[sides.index(side)] for side, w in ((0, lo), (1, hi))]
     return x, planes[0], planes[1], was_host, dims
 
 
