@@ -679,86 +679,96 @@ int validate_copies(const std::string& who, const CopyList& cl, int lo, int hi, 
   return XG_OK;
 }
 
-// The face connections' halo stage: the whole-field copy list rebased onto the slab's buffers (the field is b.in, the
-// partner b.in2), `slab_shape[0]` rows high.  The rebased pointers and shapes are built per slab, on every path (three
-// vectors of cl.n entries, small beside a slab's copies): the stage then keeps no state between slabs, so the members
-// of a host device group can run it at once.
-HaloFn copy_stage(const CopyList& cl, int dtype, int lo, int hi) {
-  return [=](const SlabBufs& b, const int64_t* slab_shape, const void*, const void* d_fill, cudaStream_t st,
-             const void** hl, const void** hh) -> int {
-    const size_t es = dtype == XG_F32 ? 4 : 8;
-    std::vector<void*> dptr(cl.n);
-    std::vector<const void*> sptr(cl.n);
-    std::vector<int64_t> shp(cl.shapes ? cl.shapes : (const int64_t*)nullptr,
-                             cl.shapes ? cl.shapes + (size_t)cl.n * cl.ndim : (const int64_t*)nullptr);
-    for (int k = 0; k < cl.n; ++k) {
-      dptr[k] = static_cast<char*>(b.plane[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
-      const void* base = cl.source[k] == kSrcField ? b.in : cl.source[k] == kSrcPartner ? b.in2 : d_fill;
-      sptr[k] = static_cast<const char*>(base) + (size_t)cl.src_offset[k] * es;
-      shp[(size_t)k * cl.ndim] = slab_shape[0];
-    }
-    if (lo) *hl = b.plane[0];
-    if (hi) *hh = b.plane[1];
-    int rc2 = xg_strided_copy_batch(dtype, cl.n, dptr.data(), sptr.data(), cl.ndim, shp.data(), cl.dst_strides,
-                                    cl.src_strides, cl.negate, st);
-    if (rc2 != XG_ENOTIMPL) return rc2;
-    for (int k = 0; k < cl.n; ++k) {  // some copy does not collapse to 5 dims: one launch per copy
-      rc2 = xg_strided_copy(dtype, dptr[k], cl.dst_strides + (size_t)k * cl.ndim, sptr[k],
-                            cl.src_strides + (size_t)k * cl.ndim, cl.ndim, shp.data() + (size_t)k * cl.ndim,
-                            cl.negate[k], st);
-      if (rc2) return rc2;
-    }
-    return XG_OK;
-  };
+// The fill constants the copy lists of a call read, in the field's dtype: the fill value of each stage, or the fill
+// value then the weight of a fill edge (1).  Pageable: cudaMemcpyAsync stages them before it returns, so they must
+// live until stencil_host / cumscan_halo_host / chain_host returns.
+struct FillConsts {
+  double f64[3];
+  float f32[3];
+  bool used = false;
+  int64_t plane_row = 0;  // of the last list checked
+  void set(int k, double v) {
+    f64[k] = v;
+    f32[k] = (float)v;
+  }
+  const void* host(int dtype) const { return used ? (dtype == XG_F32 ? (const void*)f32 : (const void*)f64) : nullptr; }
+};
+
+// The checks of a copy list that builds the halo planes of a field of `shape` padded by lo / hi along `axis`
+// (validate_copies, with the field's dim-0 row and the plane row worked out here), and fill constant k set to
+// `fill_value`.
+int check_connected(const std::string& who, const CopyList& cl, int ndim, const int64_t* shape, int axis, int lo,
+                    int hi, bool partner, int64_t partner_row, int k, double fill_value, FillConsts* fc) {
+  int64_t row_in = 1;
+  for (int d = 1; d < ndim; ++d) row_in *= shape[d];
+  fc->plane_row = shape[axis] ? row_in / shape[axis] : 0;
+  bool fill = false;
+  const int rc = validate_copies(who, cl, lo, hi, shape[0], fc->plane_row, row_in, partner, partner_row, &fill);
+  fc->used = fc->used || fill;
+  fc->set(k, fill_value);
+  return rc;
 }
 
-// The weighted face connections' halo stage: the halo of x * pre.  One xg_strided_copy_batch launch runs the copy
-// list twice: over the field into the halo planes, and over the slab's rows of the pre-metric (copy k reads it at
-// pre_offset[k] with pre_src_strides[k]; a fill copy reads the constant 1 after the fill value) into two weight planes
-// in the scratch buffer.  One xg_binary launch per padded plane then multiplies it by its weight plane in place, so
-// each halo cell is the gathered x times the gathered metric, rounded once, and a fill edge stays the fill value.
-HaloFn weighted_copy_stage(const CopyList& cl, const int64_t* pre_offset, const int64_t* pre_src_strides, int dtype,
-                           int axis, int ndim, int lo, int hi) {
+// The face connections' halo stage: the whole-field copy list rebased onto the slab's buffers (the field is b.in, the
+// partner b.in2), `slab_shape[0]` rows high, in one xg_strided_copy_batch launch.  The rebased pointers and shapes are
+// built per slab, on every path (small beside a slab's copies): the stage then keeps no state between slabs, so the
+// members of a host device group can run it at once.
+//
+// With `pre_offset` the stage builds the halo of x * pre: the batch runs the list a second time, over the slab's rows
+// of the pre-metric (copy k reads it at pre_offset[k] with pre_src_strides[k]; a fill copy reads the constant 1 after
+// the fill value) into two weight planes in the scratch buffer.  One xg_binary launch per padded plane then multiplies
+// it by its weight plane in place, so each halo cell is the gathered x times the gathered metric, rounded once, and a
+// fill edge stays the fill value.
+HaloFn copy_stage(const CopyList& cl, int dtype, int lo, int hi, const int64_t* pre_offset = nullptr,
+                  const int64_t* pre_src_strides = nullptr, int axis = 0, int ndim = 0) {
   return [=](const SlabBufs& b, const int64_t* slab_shape, const void* pre, const void* d_fill, cudaStream_t st,
              const void** hl, const void** hh) -> int {
     const size_t es = dtype == XG_F32 ? 4 : 8;
-    int64_t plane_elems = 1;
+    const size_t n = (size_t)cl.n, nd = (size_t)cl.ndim, m = pre_offset ? 2 * n : n;
+    int64_t plane_elems = 1;  // the weight planes lie side by side in the scratch buffer
     for (int d = 0; d < ndim; ++d)
       if (d != axis) plane_elems *= slab_shape[d];
-    void* weight[2] = {b.scratch, static_cast<char*>(b.scratch) + (size_t)plane_elems * es};
-    const size_t n = (size_t)cl.n, nd = (size_t)cl.ndim;
-    std::vector<void*> dptr(2 * n);
-    std::vector<const void*> sptr(2 * n);
-    std::vector<int64_t> shp(2 * n * nd), dstr(2 * n * nd), sstr(2 * n * nd);
-    std::vector<int> neg(2 * n, 0);
+    const auto weight = [&](int side) { return static_cast<char*>(b.scratch) + (size_t)side * plane_elems * es; };
+    std::vector<void*> dptr(m);
+    std::vector<const void*> sptr(m);
+    std::vector<int64_t> shp(m * nd);
     for (size_t k = 0; k < n; ++k) {
-      const bool from_fill = cl.source[k] == kSrcFill;
+      const void* base = cl.source[k] == kSrcField ? b.in : cl.source[k] == kSrcPartner ? b.in2 : d_fill;
       dptr[k] = static_cast<char*>(b.plane[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
-      sptr[k] = static_cast<const char*>(from_fill ? d_fill : b.in) + (size_t)cl.src_offset[k] * es;
-      dptr[n + k] = static_cast<char*>(weight[cl.side[k]]) + (size_t)cl.dst_offset[k] * es;
-      sptr[n + k] = from_fill ? static_cast<const char*>(d_fill) + es
-                              : static_cast<const char*>(pre) + (size_t)pre_offset[k] * es;
-      for (size_t d = 0; d < nd; ++d) {
-        shp[k * nd + d] = shp[(n + k) * nd + d] = d ? cl.shapes[k * nd + d] : slab_shape[0];
-        dstr[k * nd + d] = dstr[(n + k) * nd + d] = cl.dst_strides[k * nd + d];
-        sstr[k * nd + d] = cl.src_strides[k * nd + d];
-        sstr[(n + k) * nd + d] = pre_src_strides[k * nd + d];
-      }
-      neg[k] = cl.negate[k];
+      sptr[k] = static_cast<const char*>(base) + (size_t)cl.src_offset[k] * es;
+      for (size_t d = 0; d < nd; ++d) shp[k * nd + d] = d ? cl.shapes[k * nd + d] : slab_shape[0];
+      if (!pre_offset) continue;
+      dptr[n + k] = weight(cl.side[k]) + (size_t)cl.dst_offset[k] * es;
+      sptr[n + k] = cl.source[k] == kSrcFill ? static_cast<const char*>(d_fill) + es
+                                             : static_cast<const char*>(pre) + (size_t)pre_offset[k] * es;
+      for (size_t d = 0; d < nd; ++d) shp[(n + k) * nd + d] = shp[k * nd + d];
     }
-    int rc2 = xg_strided_copy_batch(dtype, (int)(2 * n), dptr.data(), sptr.data(), cl.ndim, shp.data(), dstr.data(),
-                                    sstr.data(), neg.data(), st);
+    // the unweighted list's strides go through as given; the weighted batch appends the metric copies' strides
+    const int64_t *dstr = cl.dst_strides, *sstr = cl.src_strides;
+    const int* neg = cl.negate;
+    std::vector<int64_t> wdstr, wsstr;
+    std::vector<int> wneg;
+    if (pre_offset) {
+      wdstr.assign(cl.dst_strides, cl.dst_strides + n * nd);
+      wdstr.insert(wdstr.end(), cl.dst_strides, cl.dst_strides + n * nd);
+      wsstr.assign(cl.src_strides, cl.src_strides + n * nd);
+      wsstr.insert(wsstr.end(), pre_src_strides, pre_src_strides + n * nd);
+      wneg.assign(cl.negate, cl.negate + n);
+      wneg.resize(2 * n, 0);
+      dstr = wdstr.data(), sstr = wsstr.data(), neg = wneg.data();
+    }
+    int rc2 = xg_strided_copy_batch(dtype, (int)m, dptr.data(), sptr.data(), cl.ndim, shp.data(), dstr, sstr, neg, st);
     if (rc2 == XG_ENOTIMPL) {  // some copy does not collapse to 5 dims: one launch per copy
       rc2 = XG_OK;
-      for (size_t k = 0; rc2 == XG_OK && k < 2 * n; ++k)
-        rc2 = xg_strided_copy(dtype, dptr[k], dstr.data() + k * nd, sptr[k], sstr.data() + k * nd, cl.ndim,
-                              shp.data() + k * nd, neg[k], st);
+      for (size_t k = 0; rc2 == XG_OK && k < m; ++k)
+        rc2 = xg_strided_copy(dtype, dptr[k], dstr + k * nd, sptr[k], sstr + k * nd, cl.ndim, shp.data() + k * nd,
+                              neg[k], st);
     }
     if (rc2) return rc2;
     const int64_t unit = 1;
-    for (int side = 0; side < 2; ++side) {
+    for (int side = 0; pre_offset && side < 2; ++side) {
       if (!(side ? hi : lo)) continue;
-      rc2 = xg_binary(XG_BIN_MUL, dtype, b.plane[side], weight[side], &unit, b.plane[side], 1, &plane_elems, st);
+      rc2 = xg_binary(XG_BIN_MUL, dtype, b.plane[side], weight(side), &unit, b.plane[side], 1, &plane_elems, st);
       if (rc2) return rc2;
     }
     if (lo) *hl = b.plane[0];
@@ -1116,13 +1126,9 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
   int rc = validate_halo_call(who.c_str(), c);
   if (rc) return rc;
   if (partner && !partner_shape) return xg_fail(XG_EINVAL, who + ": null partner shape");
-  const int64_t n0 = shape[0];
-  int64_t row_in = 1;
-  for (int d = 1; d < ndim; ++d) row_in *= shape[d];
-  const int64_t plane_row = shape[axis] ? row_in / shape[axis] : 0;
   int64_t partner_row = 0;
   if (partner) {
-    if (partner_shape[0] != n0)
+    if (partner_shape[0] != shape[0])
       return xg_fail(XG_EINVAL, who + ": the partner component's dim-0 extent differs from the field's");
     partner_row = 1;
     for (int d = 1; d < ndim; ++d) {
@@ -1130,14 +1136,11 @@ extern "C" int xg_stencil2_host_connected(int op, int dtype, const void* in, con
       partner_row *= partner_shape[d];
     }
   }
-  bool fill = false;
-  rc = validate_copies(who, cl, lo, hi, n0, plane_row, row_in, partner != nullptr, partner_row, &fill);
-  if (rc) return rc;
-  const size_t es = dtype == XG_F32 ? 4 : 8;
-  const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
-  const void* fill_host = fill ? (es == 4 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
-  return stencil_host(who.c_str(), 1, &c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
-                      fill_host);
+  FillConsts fc;
+  rc = check_connected(who, cl, ndim, shape, axis, lo, hi, partner != nullptr, partner_row, 0, fill_value, &fc);
+  return rc ? rc
+            : stencil_host(who.c_str(), 1, &c, nullptr, partner, partner_row, copy_stage(cl, dtype, lo, hi),
+                           fc.host(dtype));
 }
 
 extern "C" int xg_stencil2_host_connected_weighted(
@@ -1154,12 +1157,8 @@ extern "C" int xg_stencil2_host_connected_weighted(
   int rc = validate_halo_call(who.c_str(), c);
   if (rc) return rc;
   if (!pre_metric || !pre_strides) return xg_fail(XG_EINVAL, who + ": null pre-metric");
-  const int64_t n0 = shape[0];
-  int64_t row_in = 1;
-  for (int d = 1; d < ndim; ++d) row_in *= shape[d];
-  const int64_t plane_row = shape[axis] ? row_in / shape[axis] : 0;
-  bool fill = false;
-  rc = validate_copies(who, cl, lo, hi, n0, plane_row, row_in, false, 0, &fill);
+  FillConsts fc;
+  rc = check_connected(who, cl, ndim, shape, axis, lo, hi, false, 0, 0, fill_value, &fc);
   if (rc) return rc;
   if (ncopies > 0 && (!pre_offset || !pre_src_strides)) return xg_fail(XG_EINVAL, who + ": null pointer in the copy list");
   // the metric copies: inside the pre-metric, with its dim-0 stride, or the constant 1 at offset 0, strides 0
@@ -1182,13 +1181,10 @@ extern "C" int xg_stencil2_host_connected_weighted(
       return xg_fail(XG_EINVAL, at + "leaves the pre-metric");
     }
   }
-  // the fill value, then the weight of a fill edge (1)
-  const float f32[2] = {(float)fill_value, 1.0f};  // pageable: staged before cudaMemcpyAsync returns
-  const double f64[2] = {fill_value, 1.0};
-  const void* fill_host = fill ? (es == 4 ? (const void*)f32 : (const void*)f64) : nullptr;
+  fc.set(1, 1.0);  // the weight of a fill edge
   return stencil_host(who.c_str(), 1, &c, nullptr, nullptr, 0,
-                      weighted_copy_stage(cl, pre_offset, pre_src_strides, dtype, axis, ndim, lo, hi), fill_host, 2,
-                      2 * (size_t)plane_row * es);
+                      copy_stage(cl, dtype, lo, hi, pre_offset, pre_src_strides, axis, ndim), fc.host(dtype), 2,
+                      2 * (size_t)fc.plane_row * es);
 }
 
 extern "C" int xg_cumscan_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int axis,
@@ -1226,14 +1222,9 @@ extern "C" int xg_cumscan_host_connected(int dtype, const void* in, void* out, i
   int rc = validate_scan_call(who, s, scan_shape);
   if (rc) return rc;
   // the copies read the scanned field
-  int64_t row = 1;
-  for (int d = 1; d < ndim; ++d) row *= scan_shape[d];
-  bool fill = false;
-  rc = validate_copies(who, cl, pad_lo, pad_hi, scan_shape[0], row / scan_shape[axis], row, false, 0, &fill);
-  if (rc) return rc;
-  const float f32 = (float)fill_value;  // pageable: staged before cudaMemcpyAsync returns
-  const void* fill_host = fill ? (dtype == XG_F32 ? (const void*)&f32 : (const void*)&fill_value) : nullptr;
-  return cumscan_halo_host(who, s, scan_shape, copy_stage(cl, dtype, pad_lo, pad_hi), fill_host);
+  FillConsts fc;
+  rc = check_connected(who, cl, ndim, scan_shape, axis, pad_lo, pad_hi, false, 0, 0, fill_value, &fc);
+  return rc ? rc : cumscan_halo_host(who, s, scan_shape, copy_stage(cl, dtype, pad_lo, pad_hi), fc.host(dtype));
 }
 
 extern "C" int xg_stencil_chain_host_fold(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
@@ -1273,7 +1264,7 @@ extern "C" int xg_stencil_chain_host_connected(int dtype, const void* in, void* 
                           cs, sh);
   if (rc) return rc;
   HaloFn halo[3];
-  bool any_fill = false;
+  FillConsts fc;
   int64_t k0 = 0;  // the first copy of stage s in the concatenated lists
   for (int s = 0; s < nstage; ++s) {
     const size_t k = (size_t)k0, kd = (size_t)k0 * (size_t)(copy_ndim > 0 ? copy_ndim : 0);
@@ -1281,21 +1272,13 @@ extern "C" int xg_stencil_chain_host_connected(int dtype, const void* in, void* 
                       dst_offset ? dst_offset + k : nullptr, src_offset ? src_offset + k : nullptr,
                       shapes ? shapes + kd : nullptr, dst_strides ? dst_strides + kd : nullptr,
                       src_strides ? src_strides + kd : nullptr, negate ? negate + k : nullptr};
-    int64_t row_in = 1;
-    for (int d = 1; d < ndim; ++d) row_in *= sh[s][d];
-    const int64_t plane_row = sh[s][axis[s]] ? row_in / sh[s][axis[s]] : 0;
-    bool fill_s = false;
-    rc = validate_copies(who + ": stage " + std::to_string(s), cl, lo[s], hi[s], sh[s][0], plane_row, row_in, false,
-                         0, &fill_s);
+    rc = check_connected(who + ": stage " + std::to_string(s), cl, ndim, sh[s], axis[s], lo[s], hi[s], false, 0, s,
+                         fill[s], &fc);
     if (rc) return rc;
-    any_fill = any_fill || fill_s;
     if (lo[s] || hi[s]) halo[s] = copy_stage(cl, dtype, lo[s], hi[s]);
     k0 += cl.n;
   }
-  float f32[3];
-  for (int s = 0; s < nstage; ++s) f32[s] = (float)fill[s];  // pageable: staged before cudaMemcpyAsync returns
-  const void* fill_host = any_fill ? (dtype == XG_F32 ? (const void*)f32 : (const void*)fill) : nullptr;
-  return chain_host(who.c_str(), cs, halo, nstage, sh, fill_host);
+  return chain_host(who.c_str(), cs, halo, nstage, sh, fc.host(dtype));
 }
 
 extern "C" int xg_stencil_pair_host(int dtype, const void* a, const void* b, void* out, int ndim, const int64_t* shape,

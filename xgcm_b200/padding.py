@@ -455,10 +455,42 @@ def _unpack_vector(grid, da, other_component):
     return da, isvector, vectoraxis, da_partner
 
 
+def _require_connected_edges(grid, ax_name, lo, hi, n_face, face_offset=0):
+    """Raise when a halo of ``lo`` / ``hi`` cells along ``ax_name`` pads an edge without a face connection on one
+    of the faces ``face_offset .. face_offset + n_face - 1``: the caller has no boundary condition for such edges."""
+    face_links = grid._face_connections[grid._facedim]
+    for side, w in ((0, lo), (1, hi)):
+        if not w:
+            continue
+        unconnected = [face_offset + i for i in range(n_face)
+                       if face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side] is None]
+        if unconnected:
+            raise ValueError(
+                f"No boundary condition was specified for axis {ax_name!r}, "
+                f"but the requested operation needs to pad the {'right' if side else 'left'} "
+                f"edge of face(s) {unconnected}, which have no face "
+                f"connection there. Set a boundary condition, e.g. "
+                f"``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
+                f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
+                f"grid method."
+            )
+
+
+def _connection_sources(da, partner, x):
+    """The ``sources`` of :func:`_copy_connected_edge`: ``"self"``, the field ``da`` as the device tensor ``x``, and
+    for a vector component (``partner`` not None) ``"partner"``, the other component on ``x``'s device in its dtype."""
+    from .device import as_device_tensor
+
+    sources = {"self": (x, tuple(da.dims), [int(v) for v in x.shape], _contiguous_strides(x.shape))}
+    if partner is not None:
+        q = as_device_tensor(partner.data, x.device)[0].to(x.dtype)
+        sources["partner"] = (q, tuple(partner.dims), [int(v) for v in q.shape], _contiguous_strides(q.shape))
+    return sources
+
+
 def connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face_offset=0):
     """``(mode, fill value)`` of the unconnected edges of ``ax_name`` on a grid with face connections, after
     the same validation the simply connected path performs in ``ops.stencil2`` / ``_apply_fused_stencil``."""
-    face_links = grid._face_connections[grid._facedim]
     paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
     fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
     ax_padding = paddings[ax_name]
@@ -476,21 +508,8 @@ def connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face
         raise ValueError(
             f"padding must be one of ['periodic', 'fill', 'extend'] or None, but got {ax_padding!r}"
         )
-    for side, w in ((0, lo), (1, hi)):
-        if not w:
-            continue
-        unconnected = [face_offset + i for i in range(n_face)
-                       if face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side] is None]
-        if ax_padding is None and unconnected:
-            raise ValueError(
-                f"No boundary condition was specified for axis {ax_name!r}, "
-                f"but the requested operation needs to pad the {'right' if side else 'left'} "
-                f"edge of face(s) {unconnected}, which have no face "
-                f"connection there. Set a boundary condition, e.g. "
-                f"``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                f"grid method."
-            )
+    if ax_padding is None:
+        _require_connected_edges(grid, ax_name, lo, hi, n_face, face_offset)
     fv = fills[ax_name] if fills[ax_name] is not None else 0.0
     return (ax_padding if ax_padding is not None else "fill"), float(fv)
 
@@ -513,7 +532,7 @@ def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner
     isvector = partner_layout is not None
     cache = grid.__dict__.setdefault("_halo_plan_cache", {})
     self_strides = _contiguous_strides(shape) if self_strides is None else [int(v) for v in self_strides]
-    key = (ax_name, lo, hi, tuple(dims), tuple(shape), vectoraxis, partner_layout, tuple(self_strides))
+    key = (ax_name, lo, hi, tuple(dims), tuple(shape), vectoraxis, partner_layout, tuple(self_strides), face_offset)
     plan = cache.get(key) if remote_edges is None else None
     if plan is not None:
         return plan
@@ -546,17 +565,26 @@ def _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner
 
 
 def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=None, partner_layout=None,
-                           pre_strides=None):
+                           pre_strides=None, face_offset=0, remote_edges=None):
     """Every strided copy that builds the one-cell halo planes of a field with ``dims`` / ``shape`` along
-    ``ax_name``, for the host slab pipeline (``xg_stencil2_host_connected``), which replays the list on each
-    slab: the neighbour rims of :func:`_connected_edge_plan` plus, on each face without a connection on a
+    ``ax_name``: the neighbour rims of :func:`_connected_edge_plan` plus, on each face without a connection on a
     padded side, the basic boundary value (``mode``: fill from the constant, source ``"fill"``; extend: the
     nearest row; periodic: the row at the other end).  Each face's plane is written by exactly one copy.
+    :func:`connected_halo_planes` runs the list on device tensors; the host slab pipeline
+    (``xg_stencil2_host_connected``) replays it on each slab.
 
     ``pre_strides``: the element strides of a pre-metric read over ``shape`` (:func:`broadcast_strides`).  Each
     copy then also carries ``(pre offset, pre strides)``, the metric cells under the field cells it reads (the
     same index map over the metric; offset 0, strides 0 for a fill copy, whose weight is 1), for
-    ``xg_stencil2_host_connected_weighted``: the halo of ``x * pre``."""
+    ``xg_stencil2_host_connected_weighted``: the halo of ``x * pre``.
+
+    ``face_offset`` / ``remote_edges`` as in :func:`connected_halo_planes`: an edge whose neighbour lives in
+    another block of faces gets no copy.  The program is kept on the grid, except when ``remote_edges`` is given."""
+    cache = grid.__dict__.setdefault("_halo_program_cache", {})
+    key = (ax_name, lo, hi, tuple(dims), tuple(shape), mode, vectoraxis, partner_layout,
+           None if pre_strides is None else tuple(int(v) for v in pre_strides), face_offset)
+    if remote_edges is None and key in cache:
+        return cache[key]
     facedim = grid._facedim
     face_links = grid._face_connections[facedim]
     dims = tuple(dims)
@@ -568,17 +596,18 @@ def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=
     p_shape[t] = 1
     p_strides = _contiguous_strides(p_shape)
     loop = [d for d in range(len(dims)) if d != f]
-    program = list(_connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout))
+    program = list(_connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout,
+                                        face_offset, remote_edges))
     if pre_strides is not None:
         ms = [int(v) for v in pre_strides]
-        weights = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout,
-                                       self_strides=ms)
+        weights = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout, face_offset,
+                                       None if remote_edges is None else [], self_strides=ms)
         program = [c + (w[4], w[5]) for c, w in zip(program, weights)]
     for side, w in ((0, lo), (1, hi)):
         if not w:
             continue
         for i in range(shape[f]):
-            if face_links.get(i, {}).get(ax_name, (None, None))[side] is not None:
+            if face_links.get(face_offset + i, {}).get(ax_name, (None, None))[side] is not None:
                 continue
             c_shape = [p_shape[d] for d in loop]
             dst = (side, i * p_strides[f], [p_strides[d] for d in loop])
@@ -591,6 +620,8 @@ def connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis=
                 if pre_strides is not None:
                     weight = (i * ms[f] + row * ms[t], [ms[d] for d in loop])
             program.append(copy if pre_strides is None else copy + weight)
+    if remote_edges is None:
+        cache[key] = program
     return program
 
 
@@ -615,80 +646,52 @@ def connected_halo_planes(da, grid, ax_name, lo, hi, padding, fill_value, other_
     interior cells.  The same copies run over the metric into weight planes (1 on a fill edge, which stays the
     bare fill value, as the reference pads the already weighted array); one ``xg_binary`` launch multiplies the
     two, so each halo cell is the gathered ``x`` times the gathered metric, rounded once in the field's dtype.
+
+    The copies of :func:`connected_halo_program` (and their weight copies) go out in one
+    ``xg_strided_copy_batch`` launch.
     """
     import torch
 
     from . import ops
-    from .device import as_device_tensor
+    from .device import as_device_constant, as_device_tensor
 
-    facedim = grid._facedim
     da, isvector, vectoraxis, da_partner = _unpack_vector(grid, da, other_component)
     x, was_host = as_device_tensor(da.data, grid._device_for(da))
     dims = tuple(da.dims)
     shape = [int(v) for v in x.shape]
-    strides = _contiguous_strides(shape)
-    sources = {"self": (x, dims, shape, strides)}
-    if isvector:
-        q, _ = as_device_tensor(_strip_all_coords(da_partner).data, x.device)
-        if q.dtype != x.dtype:
-            q = q.to(x.dtype)
-        q_shape = [int(v) for v in q.shape]
-        sources["partner"] = (q, tuple(da_partner.dims), q_shape, _contiguous_strides(q_shape))
-    target_dim = _axis_dim(grid, dims, ax_name)
-    t = dims.index(target_dim)
-    n = shape[t]
-    n_face = shape[dims.index(facedim)]
-    mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, n_face, face_offset)
-    p_shape = list(shape)
-    p_shape[t] = 1
+    sources = _connection_sources(da, da_partner, x)
+    mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, shape[dims.index(grid._facedim)],
+                                   face_offset)
+    partner_layout = None if not isvector else (sources["partner"][1], tuple(sources["partner"][2]))
+    pre_strides = None
     if pre is not None:
         if isvector:
             raise NotImplementedError(
                 "metric weighting of vector components across face connections is not implemented")
         m = pre.to(x.dtype).contiguous()
-        m_strides = broadcast_strides(list(m.shape), shape)
-        # the x planes and the weight planes side by side: one product over both at the end
-        sides = [side for side, w in ((0, lo), (1, hi)) if w]
-        stack = torch.empty([2 * len(sides)] + p_shape, dtype=x.dtype, device=x.device)
-        weights = {side: stack[len(sides) + k] for k, side in enumerate(sides)}
-    planes = []
-    for side, w in ((0, lo), (1, hi)):
-        if not w:
-            planes.append(None)
-            continue
-        plane = torch.empty(p_shape, dtype=x.dtype, device=x.device) if pre is None else stack[sides.index(side)]
-        if mode == "fill":
-            plane.fill_(float(fv))
-            if pre is not None:
-                weights[side].fill_(1.0)
-        else:  # extend: nearest cell; periodic: the cell at the other end
-            if mode == "extend":
-                row = (n - 1) if side else 0
-            else:
-                assert mode == "periodic"
-                row = 0 if side else (n - 1)
-            ops.strided_copy(plane, 0, _contiguous_strides(p_shape), x, row * strides[t], strides, p_shape)
-            if pre is not None:
-                ops.strided_copy(weights[side], 0, _contiguous_strides(p_shape), m, row * m_strides[t], m_strides,
-                                 p_shape)
-        planes.append(plane)
-
-    partner_layout = None if not isvector else (sources["partner"][1], tuple(sources["partner"][2]))
-    plan = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, vectoraxis, partner_layout,
-                                face_offset, remote_edges)
-    batch = [(planes[side], doff, dstr, sources[src_key][0], soff, sstr, shp, neg)
-             for side, doff, dstr, src_key, soff, sstr, shp, neg in plan]
+        pre_strides = broadcast_strides(list(m.shape), shape)
+    program = connected_halo_program(grid, ax_name, lo, hi, dims, shape, mode, vectoraxis, partner_layout,
+                                     pre_strides, face_offset, remote_edges)
+    p_shape = list(shape)
+    p_shape[dims.index(_axis_dim(grid, dims, ax_name))] = 1
+    sides = [side for side, w in ((0, lo), (1, hi)) if w]
+    # the x planes, then the weight planes side by side: one product over both at the end
+    stack = torch.empty([len(sides) * (1 if pre is None else 2)] + p_shape, dtype=x.dtype, device=x.device)
+    planes = {side: stack[k] for k, side in enumerate(sides)}
+    tensors = {key: src[0] for key, src in sources.items()}
+    if any(c[3] == "fill" for c in program):  # the fill value, then the weight of a fill edge
+        tensors["fill"] = as_device_constant(torch.tensor([fv, 1.0], dtype=x.dtype).numpy(), x.device)
+    batch = [(planes[side], doff, dstr, tensors[src], soff, sstr, shp, neg)
+             for side, doff, dstr, src, soff, sstr, shp, neg, *_ in program]
     if pre is not None:  # the same index maps over the metric's cells
-        m_plan = _connected_edge_plan(grid, ax_name, lo, hi, dims, shape, None, None, face_offset,
-                                      [] if remote_edges is not None else None, self_strides=m_strides)
-        batch += [(weights[side], doff, dstr, m, soff, sstr, shp, False)
-                  for side, doff, dstr, _, soff, sstr, shp, _ in m_plan]
-    ops.strided_copy_batch(batch)  # both planes, every connected face (and their weights): one launch
+        batch += [(stack[len(sides) + sides.index(side)], doff, dstr, tensors["fill"] if src == "fill" else m,
+                   1 if src == "fill" else poff, pstr, shp, False)
+                  for side, doff, dstr, src, _, _, shp, _, poff, pstr in program]
+    ops.strided_copy_batch(batch)
     if pre is not None and sides:
-        n_sides = len(sides)
-        weighted = ops.binary("mul", stack[:n_sides], stack[n_sides:])
-        planes = [None if not w else weighted[sides.index(side)] for side, w in ((0, lo), (1, hi))]
-    return x, planes[0], planes[1], was_host, dims
+        weighted = ops.binary("mul", stack[:len(sides)], stack[len(sides):])
+        planes = {side: weighted[k] for k, side in enumerate(sides)}
+    return x, planes.get(0), planes.get(1), was_host, dims
 
 
 def _pad_face_connections(da, grid, padding_width, padding, fill_value, other_component=None):
@@ -698,7 +701,7 @@ def _pad_face_connections(da, grid, padding_width, padding, fill_value, other_co
     requested width with the ordinary boundary condition, (2) overwrite the halo of each
     CONNECTED edge with the neighbour's rim, always read from the pre-padded arrays, (3) trim
     back to the requested widths.  Step 2 is one batched strided-copy launch per axis.  When
-    only one axis is padded the three steps collapse into ``xg_pad`` + one batched copy.
+    one or two axes are padded the three steps collapse into ``xg_pad`` + one batched copy per axis.
 
     The reference visits the axes in ``set`` order (hash-seed dependent, padding.py:307-309);
     only halo corners depend on it.  Here the order is that of ``grid.axes``.
@@ -727,82 +730,28 @@ def _pad_face_connections(da, grid, padding_width, padding, fill_value, other_co
     face_links = connections[facedim]
     prepad_padding = dict(padding)
     for axname in pad_axes:
-        if prepad_padding.get(axname) is not None:
-            continue
-        for side, side_name in [(0, "left"), (1, "right")]:
-            if padding_width[axname][side] == 0:
-                continue
-            unconnected_faces = [
-                i for i in range(n_facedim)
-                if face_links.get(i, {}).get(axname, (None, None))[side] is None
-            ]
-            if unconnected_faces:
-                raise ValueError(
-                    f"No boundary condition was specified for axis {axname!r}, "
-                    f"but the requested operation needs to pad the {side_name} "
-                    f"edge of face(s) {unconnected_faces}, which have no face "
-                    f"connection there. Set a boundary condition, e.g. "
-                    f"``padding='fill'`` (or 'extend'/'periodic'), on the Grid "
-                    f"(``Grid(..., padding=...)``) or pass ``padding=`` to the "
-                    f"grid method."
-                )
-        # every padded edge of this axis is connected: its pre-padded halo is a placeholder
-        prepad_padding[axname] = "fill"
+        if prepad_padding.get(axname) is None:
+            _require_connected_edges(grid, axname, *padding_width[axname], n_facedim)
+            # every padded edge of this axis is connected: its pre-padded halo is a placeholder
+            prepad_padding[axname] = "fill"
 
     active = [ax for ax in pad_axes if any(padding_width[ax])]
-    if len(active) == 1:
-        # One padded axis (every built-in operator, most user ufuncs): no halo corners exist, so the
-        # three steps collapse — basic-pad that axis straight into the final shape (one pass), then
-        # overwrite the connected halos from the UNPADDED neighbours.  Same values as the general
-        # route below, two passes over the field instead of five.
-        ax = active[0]
-        lo, hi = padding_width[ax]
-        padded = _pad_basic(da, grid, {ax: (lo, hi)}, prepad_padding, fill_value)
-        out, was_host = as_device_tensor(padded.data, grid._device_for(padded))  # fresh: xg_pad allocated it
-        o_dims = tuple(padded.dims)
-        o_shape = [int(v) for v in out.shape]
-        x, _ = as_device_tensor(da.data, out.device)
-        x_shape = [int(v) for v in x.shape]
-        sources = {"self": (x, tuple(da.dims), x_shape, _contiguous_strides(x_shape))}
-        if isvector:
-            q, _ = as_device_tensor(da_partner.data, out.device)
-            if q.dtype != out.dtype:
-                q = q.to(out.dtype)
-            q_shape = [int(v) for v in q.shape]
-            sources["partner"] = (q, tuple(da_partner.dims), q_shape, _contiguous_strides(q_shape))
-        t_len = o_shape[o_dims.index(_axis_dim(grid, o_dims, ax))]
-        batch = []
-        for i in range(n_facedim):
-            links = face_links.get(i, {}).get(ax, (None, None))
-            for connection, is_right, w in ((links[0], False, lo), (links[1], True, hi)):
-                if connection and w:
-                    _copy_connected_edge(grid, facedim, out, o_dims, o_shape, i, ax, (t_len - w) if is_right else 0,
-                                         w, 0, connection, is_right, sources, isvector, vectoraxis, batch)
-        ops.strided_copy_batch(batch)
-        return DataArray(result_like(out, was_host), dims=o_dims, name=padded.name, attrs=padded.attrs)
-
-    if len(active) == 2:
-        # Two padded axes (2-D stencils of user ufuncs): still no pre-padded copies.  Basic-pad both
-        # axes straight into the final shape; then, axis by axis in the reference's order, write
-        # each connected halo slab over the FULL extent of the other axis — its corner blocks are
-        # the neighbour's own basic halo (what the reference finds in the pre-padded neighbour),
-        # produced by zero-stride / wrapped strided copies.  Two passes instead of five.
+    if len(active) in (1, 2):
+        # One padded axis (every built-in operator, most user ufuncs) or two (2-D stencils of user ufuncs): no
+        # pre-padded copies.  Basic-pad the padded axes straight into the final shape (one pass); then, axis by
+        # axis in the reference's order, overwrite the connected halos from the UNPADDED neighbours.  With two
+        # axes each halo slab spans the FULL extent of the other axis -- its corner blocks are the neighbour's
+        # own basic halo (what the reference finds in the pre-padded neighbour), produced by zero-stride /
+        # wrapped strided copies.  Same values as the general route below, two passes over the field instead
+        # of five.
         import torch
 
-        widths = {ax: padding_width[ax] for ax in active}
-        padded = _pad_basic(da, grid, widths, prepad_padding, fill_value)
+        padded = _pad_basic(da, grid, {ax: padding_width[ax] for ax in active}, prepad_padding, fill_value)
         out, was_host = as_device_tensor(padded.data, grid._device_for(padded))  # fresh: xg_pad allocated it
         o_dims = tuple(padded.dims)
         o_shape = [int(v) for v in out.shape]
         x, _ = as_device_tensor(da.data, out.device)
-        x_shape = [int(v) for v in x.shape]
-        sources = {"self": (x, tuple(da.dims), x_shape, _contiguous_strides(x_shape))}
-        if isvector:
-            q, _ = as_device_tensor(da_partner.data, out.device)
-            if q.dtype != out.dtype:
-                q = q.to(out.dtype)
-            q_shape = [int(v) for v in q.shape]
-            sources["partner"] = (q, tuple(da_partner.dims), q_shape, _contiguous_strides(q_shape))
+        sources = _connection_sources(da, da_partner, x)
         consts = {}
 
         def const(value):
@@ -813,8 +762,9 @@ def _pad_face_connections(da, grid, padding_width, padding, fill_value, other_co
 
         modes = {ax: (prepad_padding[ax], fill_value.get(ax)) for ax in pad_axes}
         for ax in active:
-            other = active[1] if ax == active[0] else active[0]
-            cross = {_axis_dim(grid, o_dims, other): padding_width[other], "modes": modes, "const": const}
+            other = next((a for a in active if a != ax), None)
+            cross = None if other is None else {_axis_dim(grid, o_dims, other): padding_width[other], "modes": modes,
+                                                "const": const}
             lo, hi = padding_width[ax]
             t_len = o_shape[o_dims.index(_axis_dim(grid, o_dims, ax))]
             batch = []
@@ -833,14 +783,8 @@ def _pad_face_connections(da, grid, padding_width, padding, fill_value, other_co
     p_dims = tuple(prepadded.dims)
     p_shape = [int(v) for v in p.shape]
     p_strides = _contiguous_strides(p_shape)
-    sources = {"self": (p, p_dims, p_shape, p_strides)}
-    if isvector:
-        partner = _pad_basic(da_partner, grid, max_padding_width, prepad_padding, fill_value)
-        q, _ = as_device_tensor(partner.data, p.device)
-        if q.dtype != p.dtype:
-            q = q.to(p.dtype)
-        q_shape = [int(v) for v in q.shape]
-        sources["partner"] = (q, tuple(partner.dims), q_shape, _contiguous_strides(q_shape))
+    partner = _pad_basic(da_partner, grid, max_padding_width, prepad_padding, fill_value) if isvector else None
+    sources = _connection_sources(prepadded, partner, p)
 
     out = p.clone()
     face_pos = p_dims.index(facedim)

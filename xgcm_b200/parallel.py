@@ -278,7 +278,7 @@ def sharded_connected_stencil2(grid, da_local, ax_name: str, op: str, lo: int, h
     block = -(-n_global // world)
     start, stop = shard_bounds(n_global, world, rank)
     raw = da_local
-    field = P._unpack_vector(grid, raw, other_component_local)[0]
+    field, isvector, vectoraxis, partner = P._unpack_vector(grid, raw, other_component_local)
     if field.sizes[facedim] != stop - start:
         raise ValueError(
             f"rank {rank} must hold faces [{start}, {stop}) along {facedim!r}, got {field.sizes[facedim]}"
@@ -291,16 +291,8 @@ def sharded_connected_stencil2(grid, da_local, ax_name: str, op: str, lo: int, h
 
     # what this rank's faces owe to other ranks: the same enumeration on every rank (global face
     # order, then side) so that sends and receives pair up
-    _, isvector, vectoraxis, partner = P._unpack_vector(grid, raw, other_component_local)
     shape = [int(v) for v in x.shape]
-    sources = {"self": (x, dims, shape, P._contiguous_strides(shape))}
-    if isvector:
-        from .device import as_device_tensor
-
-        q, _ = as_device_tensor(P._strip_all_coords(partner).data, x.device)
-        q = q.to(x.dtype)
-        q_shape = [int(v) for v in q.shape]
-        sources["partner"] = (q, tuple(partner.dims), q_shape, P._contiguous_strides(q_shape))
+    sources = P._connection_sources(field, partner, x)
     fpos = dims.index(facedim)
     tpos = dims.index(P._axis_dim(grid, dims, ax_name))
     slab_shape = list(shape)
