@@ -120,15 +120,28 @@ def test_fold_rejects_face_connections():
 
 
 @pytest.mark.parametrize("pivot", ["center", "V"])
-def test_inner_seam_position_center_pivot_raises(mock, pivot):
+def test_inner_seam_position_center_pivot_raises(mock, monkeypatch, pivot):
     ds = xg.Dataset(data_vars={"f": (("yl", "xi"), np.zeros((Ny, Nx - 1)))},
-                    coords={"xh": np.arange(Nx), "xi": np.arange(Nx - 1), "yh": np.arange(Ny), "yl": np.arange(Ny)})
+                    coords={"xh": np.arange(Nx), "xi": np.arange(Nx - 1), "yh": np.arange(Ny), "yl": np.arange(Ny),
+                            "zh": np.arange(3), "zl": np.arange(3)})
     with warnings.catch_warnings():
         warnings.simplefilter("ignore", UserWarning)
-        grid = xg.Grid(ds, coords={"X": {"center": "xh", "inner": "xi"}, "Y": {"center": "yh", "left": "yl"}},
-                       padding={"X": "periodic", "Y": {"fold": pivot}}, autoparse_metadata=False)
+        grid = xg.Grid(ds, coords={"X": {"center": "xh", "inner": "xi"}, "Y": {"center": "yh", "left": "yl"},
+                                   "Z": {"center": "zh", "left": "zl"}},
+                       padding={"X": "periodic", "Y": {"fold": pivot}, "Z": "fill"}, autoparse_metadata=False)
     with pytest.raises(NotImplementedError, match="incompatible"):
         xg.pad(ds["f"], grid, padding_width={"Y": (0, 1)})
+    # numpy fields with a batch dim in front, on a CUDA device: the slab routes cannot plan the fold either and leave
+    # the call to the whole-field route, which raises the same error (no host entry point runs: none is mocked here)
+    from xgcm_b200 import device
+
+    monkeypatch.setattr(device, "default_device", lambda: torch.device("cuda"))
+    v = xg.DataArray(np.zeros((2, Ny, Nx - 1, 3)), dims=("t", "yl", "xi", "zh"))
+    with pytest.raises(NotImplementedError, match="incompatible"):
+        grid.diff(v, "Y")
+    with pytest.raises(NotImplementedError, match="incompatible"):
+        grid.pair("diff", xg.DataArray(np.zeros((2, Ny, Nx - 1, 3)), dims=("t", "yh", "xi", "zl")), "Z", "diff", v,
+                  "Y")
 
 
 # ---------------------------------------------------------------------------------------------- oracle vs golden

@@ -18,24 +18,24 @@ CORE_FACES = ["face", "y", "x", "yl", "xl"]
 def test_route_cuts_leading_batch_dims():
     r = _host_stream_route
     # xmitgcm layouts on a face-connected grid: (time, k, face, j, i), (k, face, j, i), (1, k, face, j, i)
-    assert r("connected", ("t", "k", "face", "y", "x"), [3, 5, 6, 8, 8], CORE_FACES[:3], 0, 1) == ("connected", 0, 2)
-    assert r("connected", ("k", "face", "y", "x"), [5, 6, 8, 8], CORE_FACES[:3], 1, 1) == ("connected", 0, 1)
-    assert r("connected", ("o", "k", "face", "y", "x"), [1, 5, 6, 8, 8], CORE_FACES[:3], 1, 0) == ("connected", 1, 1)
+    assert r("connected", ("t", "k", "face", "y", "x"), [3, 5, 6, 8, 8], CORE_FACES[:3], 0, 1) == (0, 2)
+    assert r("connected", ("k", "face", "y", "x"), [5, 6, 8, 8], CORE_FACES[:3], 1, 1) == (0, 1)
+    assert r("connected", ("o", "k", "face", "y", "x"), [1, 5, 6, 8, 8], CORE_FACES[:3], 1, 0) == (1, 1)
     # NEMO (time_counter, deptht, y, x) across a fold
-    assert r("fold", ("t", "z", "y", "x"), [12, 75, 30, 40], ["y", "x"], 0, 1) == ("fold", 0, 2)
+    assert r("fold", ("t", "z", "y", "x"), [12, 75, 30, 40], ["y", "x"], 0, 1) == (0, 2)
     # a plain grid cuts its own dim 0, after dropping leading size-1 dims (it may become the operated dim)
-    assert r("plain", ("o", "z", "y", "x"), [1, 75, 24, 36], ["y"], 0, 1) == ("plain", 1, 1)
-    assert r("plain", ("o", "z", "y", "x"), [1, 75, 24, 36], ["z"], 0, 1) == ("plain", 1, 1)
-    assert r("plain", ("z", "y", "x"), [75, 24, 36], ["z"], 0, 1) == ("plain", 0, 1)
+    assert r("plain", ("o", "z", "y", "x"), [1, 75, 24, 36], ["y"], 0, 1) == (1, 1)
+    assert r("plain", ("o", "z", "y", "x"), [1, 75, 24, 36], ["z"], 0, 1) == (1, 1)
+    assert r("plain", ("z", "y", "x"), [75, 24, 36], ["z"], 0, 1) == (0, 1)
 
 
 def test_route_merges_only_what_the_metrics_allow():
     r = _host_stream_route
     dims, shape = ("t", "z", "y", "x"), [4, 5, 30, 40]
-    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(1, 1, 30, 40)]) == ("fold", 0, 2)
-    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(4, 5, 30, 40)]) == ("fold", 0, 2)
+    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(1, 1, 30, 40)]) == (0, 2)
+    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(4, 5, 30, 40)]) == (0, 2)
     # a per-level metric broadcast over time is not a reshape of (t * z): cut along t alone
-    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(1, 5, 30, 40)]) == ("fold", 0, 1)
+    assert r("fold", dims, shape, ["y", "x"], 0, 1, operand_shapes=[(1, 5, 30, 40)]) == (0, 1)
     assert _merge_leading(np.zeros((1, 1, 3, 4)), 0, 2).shape == (1, 3, 4)
     assert _merge_leading(np.zeros((1, 4, 5, 3)), 1, 2).shape == (20, 3)
 
@@ -47,9 +47,8 @@ def test_route_falls_back():
     assert r("connected", ("face", "y", "x"), [6, 8, 8], CORE_FACES[:3], 0, 1) is None
     assert r("connected", ("o", "face", "y", "x"), [1, 6, 8, 8], CORE_FACES[:3], 0, 1) is None
     assert r("fold", ("y", "x"), [30, 40], ["y", "x"], 0, 1) is None
-    # a pre-metric on a face-connected grid, a partner that cannot stream, a halo wider than one cell
+    # a partner that cannot stream, a halo wider than one cell
     dims, shape = ("t", "face", "y", "x"), [3, 6, 8, 8]
-    assert r("connected", dims, shape, CORE_FACES[:3], 0, 1, pre=True) is None
     assert r("connected", dims, shape, CORE_FACES[:3], 0, 1, partner_ok=False) is None
     assert r("fold", ("t", "y", "x"), [3, 30, 40], ["y", "x"], 0, 2) is None
 

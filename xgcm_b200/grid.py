@@ -40,6 +40,7 @@ from .grid_ufunc import (
     GridUFunc,
     _check_data_input,
     _GridUFuncSignature,
+    _halo_core_dims,
     _host_stream_route,
     _is_host_float,
     _maybe_unpack_vector_component,
@@ -655,7 +656,7 @@ class Grid:
         boundary the halo stencils do not take (extrapolate), no batch dim in front of the operated, seam and face
         dims (``_host_stream_route``), a fold the plan cannot mirror."""
         from . import ops
-        from .padding import _axis_dim, _fold_plan, connected_halo_program
+        from .padding import connected_halo_program
 
         connected = self._face_connections is not None
         if not (connected or self._folds) or not _is_host_float(array) or self._device_for(array).type != "cuda":
@@ -684,13 +685,8 @@ class Grid:
         if not connected and not any(t.folded for t, *_ in stages):
             return None
         in_dims = stages[0][1]
-        core = [t.in_dim for t, *_ in stages]
-        if connected:
-            core += [self._facedim] + [d for a in _get_all_connection_axes(self._face_connections, self._facedim)
-                                       for d in self.axes[a].coords.values() if d in in_dims]
-        else:
-            core.append(_axis_dim(self, in_dims, self._folds[next(t for t, *_ in stages if t.folded).ax_name]
-                                  ["seam_axis"]))
+        fold_axis = next((t.ax_name for t, *_ in stages if t.folded), None)
+        core = [t.in_dim for t, *_ in stages] + _halo_core_dims(self, in_dims, fold_axis)
         cut = _host_stream_route("connected" if connected else "fold", in_dims, stages[0][2], core,
                                  max(t.lo for t, *_ in stages), max(t.hi for t, *_ in stages))
         if cut is None:
@@ -702,13 +698,9 @@ class Grid:
                 specs.append((cut.axis(t.axis_num), funcname, t.lo, t.hi, mode[1]))
                 programs.append(connected_halo_program(self, t.ax_name, t.lo, t.hi, m_dims, m_shape, mode[0]))
                 continue
-            plan = None
-            if t.folded:
-                try:
-                    _, seam, skip, mirror, period = _fold_plan(self, t.ax_name, m_dims, m_shape, 1)
-                except NotImplementedError:
-                    return None
-                plan = (seam, skip, mirror, period)
+            plan = cut.fold_plan(self, t.ax_name, s_dims, s_shape) if t.folded else None
+            if t.folded and plan is None:
+                return None
             specs.append((cut.axis(t.axis_num), funcname, t.lo, t.hi, t.pad_mode if (t.lo or t.hi) else None, t.fill,
                           plan))
         x, device = cut.cut(array.data), self._host_device(array)
@@ -797,7 +789,7 @@ class Grid:
         the operated (and seam) dims stream through the GPU in slabs (``xg_stencil_pair_host``)."""
         from . import ops
         from .device import as_device_tensor, result_like
-        from .padding import _axis_dim, _fold_plan, fold_halo_planes
+        from .padding import fold_halo_planes
 
         if combine not in ("add", "sub"):
             raise ValueError(f"combine must be 'add' or 'sub', got {combine!r}")
@@ -886,18 +878,16 @@ class Grid:
             pre_a = self._metric_host(self.get_metric(fa, ma_ax), fa.dims, dt) if ma_ax else None
             pre_b = self._metric_host(self.get_metric(fb, mb_ax), fb.dims, dt) if mb_ax else None
             post = self._metric_host(self.get_metric(probe, divide_by), out_dims_a, dt) if divide_by else None
-            core = [second.in_dim, dims[-1]]
-            if second.folded:
-                core.append(_axis_dim(self, dims, self._folds[second.ax_name]["seam_axis"]))
+            core = [second.in_dim, dims[-1]] + _halo_core_dims(self, dims, second.ax_name if second.folded else None)
             cut = _host_stream_route("pair", dims, shape, core, 0, 1,
                                      operand_shapes=[m.shape for m in (pre_a, pre_b, post) if m is not None])
-            if cut is not None:
+            plan = cut.fold_plan(self, second.ax_name, dims, shape) if second.folded and cut is not None else None
+            if cut is not None and (plan is not None or not second.folded):
                 kw = dict(pre_a=cut.cut(pre_a), pre_b=cut.cut(pre_b), post=cut.cut(post), device=self._host_device(da_a))
                 spec_b = (cut.axis(spec_b[0]),) + spec_b[1:]
                 if second.folded:
-                    _, seam, skip, mirror, period = _fold_plan(self, second.ax_name, dims, shape, 1)
-                    y = ops.stencil_pair_host_fold(cut.cut(fa.data), cut.cut(fb.data), spec_a, spec_b, cut.axis(seam),
-                                                   skip, mirror, period, sub, negate=negate, **kw)
+                    y = ops.stencil_pair_host_fold(cut.cut(fa.data), cut.cut(fb.data), spec_a, spec_b, *plan, sub,
+                                                   negate=negate, **kw)
                 else:
                     y = ops.stencil_pair_host(cut.cut(fa.data), cut.cut(fb.data), spec_a, spec_b, sub, **kw)
                 return finish(y.reshape(shape))
@@ -1092,7 +1082,7 @@ class Grid:
         cumint and metric_weighted, a per-side padding mapping, no batch dim in front of the halo dims, a fold the
         plan cannot mirror)."""
         from . import ops
-        from .padding import _axis_dim, _fold_plan, connected_halo_program
+        from .padding import connected_halo_program
 
         bc, fv, halo = s.bc, s.fill, None  # halo: the fold or face connection the padded edge crosses
         if self._face_connections is not None or s.ax_name in self._folds:
@@ -1126,12 +1116,7 @@ class Grid:
             y = ops.cumscan_host(x, axis_num, s.reverse, s.trim, s.pad_lo, s.pad_hi, bc, fv, pre=pre, post=post,
                                  skipna=True, device=device)
         else:
-            if halo == "fold":
-                core = [s.dim, _axis_dim(self, dims, self._folds[s.ax_name]["seam_axis"])]
-            else:
-                core = [s.dim, self._facedim] + [d for a in _get_all_connection_axes(self._face_connections,
-                                                                                       self._facedim)
-                                                 for d in self.axes[a].coords.values() if d in dims]
+            core = [s.dim] + _halo_core_dims(self, dims, s.ax_name)
             cut = _host_stream_route(halo, dims, shape, core, s.pad_lo, s.pad_hi,
                                      operand_shapes=[m.shape for m in (pre, post) if m is not None])
             if cut is None:
@@ -1141,12 +1126,10 @@ class Grid:
             m_dims, m_scanned = cut.dims(dims), cut.shape(scanned)
             kw = dict(pre=cut.cut(pre), post=cut.cut(post), skipna=True, device=device)
             if halo == "fold":
-                try:
-                    _, seam, skip, mirror, period = _fold_plan(self, s.ax_name, m_dims, m_scanned, 1)
-                except NotImplementedError:
+                plan = cut.fold_plan(self, s.ax_name, dims, scanned)
+                if plan is None:
                     return None
-                y = ops.cumscan_host_fold(cut.cut(x), cut.axis(axis_num), s.reverse, s.trim, seam, skip, mirror,
-                                          period, **kw)
+                y = ops.cumscan_host_fold(cut.cut(x), cut.axis(axis_num), s.reverse, s.trim, *plan, **kw)
             else:
                 mode, fv = connected_edge_mode(self, s.ax_name, s.pad_lo, s.pad_hi, padding, fill_value,
                                                shape[dims.index(self._facedim)])

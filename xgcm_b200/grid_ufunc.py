@@ -26,7 +26,7 @@ from typing import Any, Callable, Dict, List, Mapping, NamedTuple, Optional, Seq
 import numpy as np
 
 from .labeled import DataArray
-from .padding import fold_edges, missing_boundary_error, pad
+from .padding import _axis_dim, _fold_plan, _get_all_connection_axes, fold_edges, missing_boundary_error, pad
 
 _AXIS_NAME = r"\w+"
 _AXIS_POSITION = "(?:center|left|right|inner|outer)"
@@ -517,9 +517,8 @@ def apply_as_grid_ufunc(
     if fused:
         results = (
             _apply_fused_stencil(
-                kernel_op, input_arrays[0], grid, axis[0][0], in_core_dims[0][0],
-                out_core_dims[0][0], padding_width_real, padding, fill_value,
-                pre_metric, post_metric_fn, raw_arg=args[0], other_component=other_component[0],
+                kernel_op, input_arrays[0], args[0], other_component[0], grid, axis[0][0], in_core_dims[0][0],
+                out_core_dims[0][0], padding_width_real, padding, fill_value, pre_metric, post_metric_fn,
             ),
         )
     else:
@@ -538,126 +537,109 @@ def apply_as_grid_ufunc(
     return results
 
 
-def _apply_connected_stencil(op, da, raw_arg, other_component, grid, ax_name, in_dim, out_dim,
-                             padding_width_real, padding, fill_value, pre_metric, post_metric_fn):
-    """Built-in operator on a grid with face connections: the halo is not an affine function of
-    the field any more (it comes from other faces, rotated).  A one-cell halo is gathered into thin
-    planes (``connected_halo_planes``, of ``x * pre`` under a pre-metric) that the fused stencil takes
-    beside the field; a numpy field streams in slabs that do the same.  A wider halo (user ufuncs) is
-    materialised by ``pad`` and the stencil runs on the padded array without a boundary condition
-    (reference: grid_ufunc.py:903-921 pads, then applies the kernel)."""
+def _apply_fused_stencil(op, da, raw_arg, other_component, grid, ax_name, in_dim, out_dim, padding_width_real,
+                         padding, fill_value, pre_metric, post_metric_fn):
+    """One ``xg_stencil2`` launch: halo + operator + metric weighting.  Across a north fold or a face connection the
+    one-cell halo is not a boundary condition of the field: it comes in as thin planes beside it, the folded row
+    (``fold_halo_planes``) or the rims of the neighbour faces, rotated (``connected_halo_planes``), both of
+    ``x * pre`` under a pre-metric.  A numpy field streams through the host slab pipeline that builds the same planes
+    per slab.  A wider halo across face connections (user ufuncs) is materialised by ``pad`` and the stencil runs on
+    the padded array without a boundary condition (reference: grid_ufunc.py:903-921 pads, then applies the kernel)."""
     from . import ops
     from .device import as_device_tensor, result_like
-    from .padding import pad
+    from .padding import (_unpack_vector, broadcast_strides, connected_edge_mode, connected_halo_planes,
+                          connected_halo_program, fold_halo_planes)
 
     lo, hi = padding_width_real.get(ax_name, (0, 0))
-    if pre_metric is not None and isinstance(raw_arg, dict):
-        raise NotImplementedError(
-            "metric weighting of vector components across face connections is not implemented"
-        )
-    if lo <= 1 and hi <= 1:
-        streamed = _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi,
-                                             padding, fill_value, post_metric_fn, pre_metric)
-        if streamed is not None:
-            return streamed
-        # halo planes gathered from the neighbour faces (of x * pre), then the ordinary fused launch
-        from .padding import connected_halo_planes
-
-        arg, pre_t, was_host = raw_arg, None, None
-        if pre_metric is not None:
-            x, was_host = as_device_tensor(da.data, grid._device_for(da))
-            pre_t = grid._metric_tensor(pre_metric, da.dims, x)
-            arg = DataArray(x, dims=da.dims, name=da.name, attrs=da.attrs)
-        x, halo_lo, halo_hi, on_host, dims = connected_halo_planes(
-            arg, grid, ax_name, lo, hi, padding, fill_value, other_component, pre=pre_t)
-        was_host = on_host if was_host is None else was_host
-        axis_num = dims.index(in_dim)
-        out_dims = tuple(out_dim if d == in_dim else d for d in dims)
-        out_shape = list(x.shape)
-        out_shape[axis_num] = x.shape[axis_num] + lo + hi - 1
-        post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
-        post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
-        out = ops.stencil2(x, axis_num, op, lo, hi, "fill" if (lo or hi) else None, 0.0,
-                           pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
-        return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
-    if pre_metric is not None:
-        raise NotImplementedError(
-            "metric weighting across face connections takes a halo of at most one cell per side"
-        )
-    padded = pad(raw_arg, grid=grid, padding_width={ax_name: (lo, hi)}, padding=padding,
-                 fill_value=fill_value, other_component=other_component)
-    if isinstance(padded, dict):  # zero-width request: pad returns its input untouched
-        [padded] = list(padded.values())
-    axis_num = padded.get_axis_num(in_dim)
-    out_dims = tuple(out_dim if d == in_dim else d for d in padded.dims)
-    out_shape = list(padded.shape)
-    out_shape[axis_num] = padded.shape[axis_num] - 1
+    dims, shape = tuple(da.dims), list(da.shape)
+    connected, vector = grid._face_connections is not None, isinstance(raw_arg, dict)
+    folded, partner = False, None
+    if connected:
+        if pre_metric is not None and vector:
+            raise NotImplementedError(
+                "metric weighting of vector components across face connections is not implemented"
+            )
+        if lo > 1 or hi > 1:
+            if pre_metric is not None:
+                raise NotImplementedError(
+                    "metric weighting across face connections takes a halo of at most one cell per side"
+                )
+            padded = _maybe_unpack_vector_component(pad(raw_arg, grid=grid, padding_width={ax_name: (lo, hi)},
+                                                        padding=padding, fill_value=fill_value,
+                                                        other_component=other_component))
+            axis_num = padded.get_axis_num(in_dim)
+            out_dims = tuple(out_dim if d == in_dim else d for d in padded.dims)
+            out_shape = list(padded.shape)
+            out_shape[axis_num] -= 1
+            post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
+            x, was_host = as_device_tensor(padded.data, grid._device_for(padded))
+            post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
+            out = ops.stencil2(x, axis_num, op, 0, 0, None, post=post_t)
+            return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
+        _, _, vectoraxis, partner = _unpack_vector(grid, raw_arg, other_component)
+        mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, shape[dims.index(grid._facedim)])
+    else:
+        paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
+        fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
+        folded, mode, fv = _stencil_boundary(grid, ax_name, lo, hi, paddings, fills)
+    bc = mode if (lo or hi) else None
+    axis_num = dims.index(in_dim)
+    out_dims = tuple(out_dim if d == in_dim else d for d in dims)
+    out_shape = list(shape)
+    out_shape[axis_num] += lo + hi - 1
     post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
-    x, was_host = as_device_tensor(padded.data, grid._device_for(padded))
-    post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
-    out = ops.stencil2(x, axis_num, op, 0, 0, None, post=post_t)
-    return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
 
-
-def _apply_fused_stencil(op, da, grid, ax_name, in_dim, out_dim, padding_width_real, padding,
-                         fill_value, pre_metric, post_metric_fn, raw_arg=None, other_component=None):
-    """One ``xg_stencil2`` launch: halo + operator + metric weighting."""
-    from . import ops
-    from .device import as_device_tensor, result_like
-
-    if grid._face_connections is not None:
-        return _apply_connected_stencil(
-            op, da, da if raw_arg is None else raw_arg, other_component, grid, ax_name, in_dim,
-            out_dim, padding_width_real, padding, fill_value, pre_metric, post_metric_fn,
-        )
-    from .padding import fold_halo_planes
-
-    lo, hi = padding_width_real.get(ax_name, (0, 0))
-    paddings = grid._complete_user_kwargs_using_axis_defaults(padding, "padding")
-    fills = grid._complete_user_kwargs_using_axis_defaults(fill_value, "fill_value")
-    folded, ax_padding, fv = _stencil_boundary(grid, ax_name, lo, hi, paddings, fills)
-    axis_num = da.get_axis_num(in_dim)
-    out_dims = tuple(out_dim if d == in_dim else d for d in da.dims)
-    out_shape = list(da.shape)
-    out_shape[axis_num] = da.shape[axis_num] + lo + hi - 1
-    post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
-    bc = ax_padding if (lo or hi) else None
-
-    if _is_host_float(da) and (not folded or grid._device_for(da).type == "cuda"):
-        # host field: stream slabs H2D -> kernel -> D2H inside the library (xg_stencil2_host, or
-        # xg_stencil2_host_fold with the folded row of each slab as its north halo)
-        dims, shape = tuple(da.dims), list(da.shape)
+    # a numpy field streams in slabs H2D -> halo planes -> kernel -> D2H inside the library; the halo planes are
+    # CUDA launches, so a fold or face-connected field streams only from a CUDA device
+    if _is_host_float(da) and (not (connected or folded) or grid._device_for(da).type == "cuda"):
         pre_h = None if pre_metric is None else grid._metric_host(pre_metric, dims, da.data.dtype)
         post_h = None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype)
-        core = [in_dim]
-        if folded:
-            from .padding import _axis_dim, _fold_plan
-
-            core.append(_axis_dim(grid, dims, grid._folds[ax_name]["seam_axis"]))
-        cut = _host_stream_route("fold" if folded else "plain", dims, shape, core, lo, hi,
+        core = [in_dim] + (_halo_core_dims(grid, dims, ax_name) if (connected or folded) else [])
+        partner_ok = True
+        if partner is not None:  # the other vector component streams beside the field, cut the same way
+            first = min(dims.index(d) for d in core)
+            partner_ok = (not partner.is_device and isinstance(partner.data, np.ndarray)
+                          and len(partner.dims) == len(dims) and tuple(partner.dims[:first]) == dims[:first]
+                          and tuple(partner.shape[:first]) == tuple(shape[:first]))
+        cut = _host_stream_route("connected" if connected else "fold" if folded else "plain", dims, shape, core,
+                                 lo, hi, partner_ok=partner_ok,
                                  operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
-        if cut is not None:
-            kw = dict(pre=cut.cut(pre_h), post=cut.cut(post_h), device=grid._host_device(da))
+        plan = cut.fold_plan(grid, ax_name, dims, shape) if folded and cut is not None else None
+        if cut is not None and (plan is not None or not folded):
+            x, axis, pre_m = cut.cut(da.data), cut.axis(axis_num), cut.cut(pre_h)
+            kw = dict(post=cut.cut(post_h), device=grid._host_device(da))
             try:
-                if folded:
-                    _, seam, skip, mirror, period = _fold_plan(grid, ax_name, dims, shape, 1)
-                    out = ops.stencil2_host_fold(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, bc, fv,
-                                                 cut.axis(seam), skip, mirror, period,
-                                                 negate=isinstance(raw_arg, dict), **kw)
+                if connected:
+                    m_dims, m_shape = cut.dims(dims), cut.shape(shape)
+                    if pre_m is not None:  # a scalar field: vector components with a pre-metric raised above
+                        program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode,
+                                                         pre_strides=broadcast_strides(pre_m.shape, m_shape))
+                        out = ops.stencil2_host_connected_weighted(x, axis, op, lo, hi, fv, program, pre=pre_m, **kw)
+                    else:
+                        q = None if partner is None else cut.cut(partner.data)
+                        layout = None if partner is None else (cut.dims(partner.dims), tuple(q.shape))
+                        program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode, vectoraxis,
+                                                         layout)
+                        out = ops.stencil2_host_connected(x, axis, op, lo, hi, fv, program, partner=q, **kw)
+                elif folded:
+                    out = ops.stencil2_host_fold(x, axis, op, lo, hi, bc, fv, *plan, negate=vector, pre=pre_m, **kw)
                 else:
-                    out = ops.stencil2_host(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, bc, fv, **kw)
+                    out = ops.stencil2_host(x, axis, op, lo, hi, bc, fv, pre=pre_m, **kw)
                 return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
             except NotImplementedError:
                 pass  # e.g. periodic halo + pre-metric along the outermost axis: whole-field path below
 
     x, was_host = as_device_tensor(da.data, grid._device_for(da))
-    pre_t = grid._metric_tensor(pre_metric, da.dims, x) if pre_metric is not None else None
-    post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
+    pre_t = grid._metric_tensor(pre_metric, dims, x) if pre_metric is not None else None
     halo_lo = halo_hi = None
-    if folded:
-        # the north halo is the folded row of x * pre, sign-flipped for a vector component
-        halo_lo, halo_hi = fold_halo_planes(grid, ax_name, da.dims, x, lo, ax_padding, pre=pre_t,
-                                            negate=isinstance(raw_arg, dict))
+    if connected:  # the planes replace both padded edges: the boundary condition is a placeholder
+        field = da._replace(data=x)
+        x, halo_lo, halo_hi, _, _ = connected_halo_planes({vectoraxis: field} if vector else field, grid, ax_name,
+                                                          lo, hi, padding, fill_value, other_component, pre=pre_t)
+        bc, fv = ("fill" if (lo or hi) else None), 0.0
+    elif folded:  # the north halo is the folded row of x * pre, sign-flipped for a vector component
+        halo_lo, halo_hi = fold_halo_planes(grid, ax_name, dims, x, lo, mode, pre=pre_t, negate=vector)
+    post_t = grid._metric_tensor(post_da, out_dims, x) if post_da is not None else None
     out = ops.stencil2(x, axis_num, op, lo, hi, bc, fv, pre=pre_t, post=post_t, halo_lo=halo_lo, halo_hi=halo_hi)
     return DataArray(result_like(out, was_host), dims=out_dims, name=da.name, attrs=da.attrs)
 
@@ -680,7 +662,6 @@ class HostCut(NamedTuple):
     """How a numpy field is cut into slabs along dim 0 (``_host_stream_route``): its first ``ndrop`` dims (of
     extent 1) are dropped and the next ``nmerge`` merged into one dim 0, the slab dim."""
 
-    kind: str
     ndrop: int
     nmerge: int
 
@@ -702,26 +683,50 @@ class HostCut(NamedTuple):
         lead = self.ndrop + self.nmerge
         return [int(np.prod(shape[self.ndrop:lead]))] + [int(v) for v in shape[lead:]]
 
+    def fold_plan(self, grid, ax_name, dims, shape):
+        """``(seam dim, skip, mirror, period)`` of the one-row north halo across the fold of ``ax_name`` of a field
+        with ``dims`` / ``shape``, planned as the whole-field route plans it, the seam dim in the merged layout.  None
+        when the plan cannot mirror (an ``inner`` seam under a center pivot): the whole-field route raises that
+        error."""
+        try:
+            _, seam, skip, mirror, period = _fold_plan(grid, ax_name, dims, shape, 1)
+        except NotImplementedError:
+            return None
+        return self.axis(seam), skip, mirror, period
 
-def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_ok=True, operand_shapes=()):
+
+def _halo_core_dims(grid, dims, fold_axis=None):
+    """The dims of ``dims`` that a one-cell halo reads beside the operated dims, which the slabs of a numpy field must
+    not cut (``_host_stream_route``): on a grid with face connections the face dim and the dims of every connection
+    axis; across the north fold of ``fold_axis`` its seam dim; otherwise none."""
+    if grid._face_connections is not None:
+        facedim = grid._facedim
+        return [facedim] + [d for a in _get_all_connection_axes(grid._face_connections, facedim)
+                            for d in grid.axes[a].coords.values() if d in dims]
+    if fold_axis is not None:
+        return [_axis_dim(grid, dims, grid._folds[fold_axis]["seam_axis"])]
+    return []
+
+
+def _host_stream_route(kind, dims, shape, core_dims, lo, hi, partner_ok=True, operand_shapes=()):
     """Whether a numpy field streams through a host slab pipeline, and how it is cut.
 
     ``kind``: "plain" (``xg_stencil2_host``), "fold" (the operator crosses a north fold), "connected" (face
     connections) or "pair" (``xg_stencil_pair_host`` and its fold variant); ``core_dims``: the dims the
-    operator or any halo source indexes (operated dims; seam dim; face dim and the dims of the connection
-    axes).  The slabs are cut along dim 0: leading size-1 dims are dropped first, then the leading batch dims
-    (those before the first core dim) are merged into one dim 0 -- as far as every broadcast operand (metric
-    ``operand_shapes``, 1 where it broadcasts) merges with them.  A plain grid cuts the field's own dim 0 (no
-    merge), which may be the operated dim.  Returns the :class:`HostCut`, or None for the whole-field device
-    path: a fold, connected or pair field with no batch dim in front, a halo wider than one cell, a pre-metric
-    or a partner component that cannot stream beside the field on a connected grid."""
+    operator or any halo source indexes (operated dims and :func:`_halo_core_dims`).  The slabs are cut along dim
+    0: leading size-1 dims are dropped first, then the leading batch dims (those before the first core dim) are
+    merged into one dim 0 -- as far as every broadcast operand (metric ``operand_shapes``, 1 where it broadcasts)
+    merges with them.  A plain grid cuts the field's own dim 0 (no merge), which may be the operated dim.  Returns
+    the :class:`HostCut`, or None for the whole-field device path: a fold, connected or pair field with no batch
+    dim in front, a halo wider than one cell, or a partner component that cannot stream beside the field on a
+    connected grid."""
     first = min(list(dims).index(d) for d in core_dims)
     ndrop = 0
     while ndrop < first and shape[ndrop] == 1:
         ndrop += 1
     if kind == "plain":
-        return HostCut(kind, ndrop, 1)
-    if lo > 1 or hi > 1 or first == ndrop or (kind == "connected" and (pre or not partner_ok)):
+        return HostCut(ndrop, 1)
+    if lo > 1 or hi > 1 or first == ndrop or (kind == "connected" and not partner_ok):
         return None
     nmerge = first - ndrop
 
@@ -731,7 +736,7 @@ def _host_stream_route(kind, dims, shape, core_dims, lo, hi, pre=False, partner_
 
     while nmerge > 1 and not all(merges(m, nmerge) for m in operand_shapes):
         nmerge -= 1
-    return HostCut(kind, ndrop, nmerge)
+    return HostCut(ndrop, nmerge)
 
 
 def _merge_leading(a, ndrop, nmerge):
@@ -739,57 +744,6 @@ def _merge_leading(a, ndrop, nmerge):
     the next ``nmerge`` merged into one (``_host_stream_route`` checked that this is a reshape)."""
     a = np.ascontiguousarray(a)
     return a.reshape((int(np.prod(a.shape[ndrop:ndrop + nmerge])),) + a.shape[ndrop + nmerge:])
-
-
-def _stream_connected_stencil(op, raw_arg, other_component, grid, ax_name, in_dim, out_dim, lo, hi, padding,
-                              fill_value, post_metric_fn, pre_metric=None):
-    """A built-in operator on a numpy field of a grid with face connections through the host slab pipeline
-    (``xg_stencil2_host_connected``, or ``xg_stencil2_host_connected_weighted`` with a ``pre_metric`` on a scalar
-    field), or None when the field does not stream (``_host_stream_route``)."""
-    from . import ops
-    from .padding import (_get_all_connection_axes, _unpack_vector, broadcast_strides, connected_edge_mode,
-                          connected_halo_program)
-
-    da, isvector, vectoraxis, partner = _unpack_vector(grid, raw_arg, other_component)
-    if not _is_host_float(da) or grid._device_for(da).type != "cuda":
-        return None
-    dims, shape = tuple(da.dims), [int(v) for v in da.shape]
-    facedim = grid._facedim
-    core = [in_dim, facedim]
-    for axname in _get_all_connection_axes(grid._face_connections, facedim):
-        core += [d for d in grid.axes[axname].coords.values() if d in dims]
-    mode, fv = connected_edge_mode(grid, ax_name, lo, hi, padding, fill_value, shape[dims.index(facedim)])
-    axis_num = dims.index(in_dim)
-    out_dims = tuple(out_dim if d == in_dim else d for d in dims)
-    out_shape = list(shape)
-    out_shape[axis_num] = shape[axis_num] + lo + hi - 1
-    post_da = post_metric_fn(_ShapeProbe(out_dims, out_shape)) if post_metric_fn is not None else None
-    post_h = None if post_da is None else grid._metric_host(post_da, out_dims, da.data.dtype)
-    pre_h = None if pre_metric is None else grid._metric_host(pre_metric, dims, da.data.dtype)
-    first = min(dims.index(d) for d in core)
-    partner_ok = not isvector or (
-        not partner.is_device and isinstance(partner.data, np.ndarray) and len(partner.dims) == len(dims)
-        and tuple(partner.dims[:first]) == dims[:first] and tuple(partner.shape[:first]) == tuple(shape[:first]))
-    cut = _host_stream_route("connected", dims, shape, core, lo, hi, partner_ok=partner_ok,
-                             operand_shapes=[m.shape for m in (pre_h, post_h) if m is not None])
-    if cut is None:
-        return None
-    m_dims, m_shape = cut.dims(dims), cut.shape(shape)
-    kw = dict(post=cut.cut(post_h), device=grid._host_device(da))
-    if pre_h is not None:  # a scalar field (vector components with a pre-metric raise before this)
-        pre_m = cut.cut(pre_h)
-        program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode,
-                                         pre_strides=broadcast_strides(pre_m.shape, m_shape))
-        out = ops.stencil2_host_connected_weighted(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program,
-                                                   pre=pre_m, **kw)
-        return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
-    q = partner_layout = None
-    if isvector:
-        q = cut.cut(partner.data)
-        partner_layout = (cut.dims(partner.dims), tuple(q.shape))
-    program = connected_halo_program(grid, ax_name, lo, hi, m_dims, m_shape, mode, vectoraxis, partner_layout)
-    out = ops.stencil2_host_connected(cut.cut(da.data), cut.axis(axis_num), op, lo, hi, fv, program, partner=q, **kw)
-    return DataArray(out.reshape(out_shape), dims=out_dims, name=da.name, attrs=da.attrs)
 
 
 class _ShapeProbe:
