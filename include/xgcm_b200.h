@@ -138,6 +138,23 @@ XG_API int xg_stencil_multi(int dtype, const void* in, void* out, int ndim, cons
                      const int* bc, const double* fill_value, void* stream);
 
 /*
+ * xg_stencil_multi with per-stage metrics (Grid.diff / interp / min / max over several axes with
+ * metric_weighted): stage k computes  u_{k+1} = OP_k(pad_k(u_k * pre[k])) / post[k],  bit for bit the chain of
+ * xg_stencil2 calls with pre / post metrics (every product, operator and quotient rounded to the field dtype; a
+ * fill halo is the bare fill value, a periodic / extend halo the weighted value of its source).  pre[k] / post[k]
+ * (may be NULL, as may the arrays themselves: an unweighted stage) are device arrays of the field dtype addressed
+ * with element strides pre_strides[k * ndim + d] against the stage's input shape and post_strides[k * ndim + d]
+ * against its output shape (0: broadcast).  A negative stride along a dim of extent > 1 gives XG_EINVAL; a layout
+ * with two or more non-operated dims after the last operated one XG_ENOTIMPL.  One launch, labelled
+ * "xg_stencil_multi(weighted)" (the register-staged kernel; the TMA-staged form takes no metrics).
+ */
+XG_API int xg_stencil_multi_weighted(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                              int naxes, const int* axes, const int* ops, const int* lo, const int* hi,
+                              const int* bc, const double* fill_value, const void* const* pre,
+                              const int64_t* pre_strides, const void* const* post, const int64_t* post_strides,
+                              void* stream);
+
+/*
  * Two-FIELD composite in one pass (SURVEY 8f N1: divergence, vorticity ...):
  *   out = ( OPa(pad_a(a * pre_a)) along the INNERMOST dim  (+ | -)  OPb(pad_b(b * pre_b)) along axis_b ) / post
  * a, b, out and every metric are laid out against the one common `shape` (both stencils are length
@@ -551,6 +568,17 @@ XG_API int xg_vinterp_conservative_host(int dtype, const void* phi, const void* 
 XG_API int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
                                  const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
                                  const double* fill_value, int device);
+
+/*
+ * Host-buffer twin of xg_stencil_multi_weighted: the slabs, boundaries and refusals of xg_stencil_multi_host, with
+ * HOST metric arrays uploaded whole, once per device, and each slab's launch offset into them.  Every argument is
+ * checked before any CUDA call.
+ */
+XG_API int xg_stencil_multi_weighted_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                          int naxes, const int* axes, const int* ops, const int* lo, const int* hi,
+                                          const int* bc, const double* fill_value, const void* const* pre,
+                                          const int64_t* pre_strides, const void* const* post,
+                                          const int64_t* post_strides, int device);
 
 /*
  * Weighted sum (XG_REDUCE_SUM) or mean (XG_REDUCE_MEAN) of a HOST field over the `naxes` >= 2 distinct dims

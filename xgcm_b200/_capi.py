@@ -48,6 +48,11 @@ SIGNATURES = {
         [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int),
          C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_double), _vp],
     ),
+    "xg_stencil_multi_weighted": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, _i32p, _i32p, _i32p, _i32p, _i32p, _f64p,
+         _vpp, _i64p, _vpp, _i64p, _vp],
+    ),
     "xg_cumscan": (
         C.c_int,
         [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
@@ -151,6 +156,11 @@ SIGNATURES = {
     "xg_stencil_multi_host": (
         C.c_int,
         [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, _i32p, _i32p, _i32p, _i32p, _i32p, _f64p, C.c_int],
+    ),
+    "xg_stencil_multi_weighted_host": (
+        C.c_int,
+        [C.c_int, _vp, _vp, C.c_int, _i64p, C.c_int, _i32p, _i32p, _i32p, _i32p, _i32p, _f64p,
+         _vpp, _i64p, _vpp, _i64p, C.c_int],
     ),
     "xg_wreduce_host_multi": (
         C.c_int,

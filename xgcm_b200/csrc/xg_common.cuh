@@ -96,6 +96,12 @@ int xg_collapse_view(int ndim, const int64_t* shape, int axis, XgView* v);
 int xg_make_operand(const void* ptr, const int64_t* strides, int ndim,
                     const int64_t* shape, int axis, int vec, size_t elem_size,
                     XgOperand* op, const char* what);
+// host: every argument check of xg_stencil_multi[_weighted][_host] (error text prefixed with `who`); the metric
+// arrays may be null
+int xg_stencil_multi_check(const char* who, int dtype, const void* in, const void* out, int ndim,
+                           const int64_t* shape, int naxes, const int* axes, const int* ops, const int* lo,
+                           const int* hi, const int* bc, const double* fill_value, const void* const* pre,
+                           const int64_t* pre_strides, const void* const* post, const int64_t* post_strides);
 
 __host__ __device__ __forceinline__ int64_t xg_groups_offset(const XgGroups& g,
                                                              int64_t flat) {

@@ -27,7 +27,8 @@ enum Aux {
   kAuxThetaBounds,  // its bounds, made on the device from centres
   kAuxTarget,       // target levels of xg_vinterp_linear_host, or the bins of xg_vinterp_conservative_host
   kAuxPartial,      // per-slab partials of xg_wreduce_host_multi over every dim, and what their last launches make
-  kNumAux
+  kAuxStage0,       // pre-metrics of the stages of xg_stencil_multi_weighted_host (3 slots), then their post-metrics
+  kNumAux = kAuxStage0 + 6
 };
 
 // [C][L][R] view of a C-contiguous array around the slab dimension (extent L)

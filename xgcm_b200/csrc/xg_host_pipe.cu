@@ -224,24 +224,16 @@ TransformViews transform_views(int ndim, const int64_t* shape, int axis, int64_t
 }  // namespace
 
 // ---------------------------------------------------------------------------------------------------
-extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
-                                     const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
-                                     const double* fill_value, int device) {
-  const std::string who = "xg_stencil_multi_host";
-  if (!in || !out || !shape || !axes || !ops || !lo || !hi || !bc || !fill_value)
-    return xg_fail(XG_EINVAL, who + ": null pointer");
-  if (ndim < 1 || ndim > XG_MAX_NDIM) return xg_fail(XG_EINVAL, who + ": bad ndim");
-  if (naxes < 2 || naxes > 3) return xg_fail(XG_EINVAL, who + ": 2 or 3 axes (use xg_stencil2 for one)");
-  for (int k = 0; k < naxes; ++k) {
-    if (ops[k] < XG_OP_DIFF || ops[k] > XG_OP_MAX) return xg_fail(XG_EINVAL, who + ": unknown op");
-    if (ops[k] != ops[0])
-      return xg_fail(XG_ENOTIMPL, who + ": the fused kernel applies ONE operator along all axes "
-                                        "(what Grid.diff / interp / min / max do); chain xg_stencil2 for mixed ones");
-  }
-  if (in == out) return xg_fail(XG_EINVAL, who + ": in-place operation is not supported");
-  if (dtype != XG_F32 && dtype != XG_F64) return xg_fail(XG_EINVAL, who + ": dtype must be XG_F32 or XG_F64");
-  for (int d = 0; d < ndim; ++d)
-    if (shape[d] < 0) return xg_fail(XG_EINVAL, who + ": negative extent");
+namespace {
+
+int multi_host(const char* name, int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
+               const int* axes, const int* ops, const int* lo, const int* hi, const int* bc, const double* fill_value,
+               const void* const* pre, const int64_t* pre_strides, const void* const* post,
+               const int64_t* post_strides, int device) {
+  const std::string who = name;
+  int rc = xg_stencil_multi_check(name, dtype, in, out, ndim, shape, naxes, axes, ops, lo, hi, bc, fill_value, pre,
+                                  pre_strides, post, post_strides);
+  if (rc) return rc;
   int app[XG_MAX_NDIM];  // application index of each dim, -1 where it is not operated
   int64_t out_shape[XG_MAX_NDIM];
   for (int d = 0; d < ndim; ++d) {
@@ -249,16 +241,8 @@ extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int n
     out_shape[d] = shape[d];
   }
   for (int k = 0; k < naxes; ++k) {
-    const int d = axes[k];
-    if (d < 0 || d >= ndim) return xg_fail(XG_EINVAL, who + ": axis out of range");
-    if (app[d] >= 0) return xg_fail(XG_EINVAL, who + ": an axis may appear only once");
-    if (lo[k] < 0 || lo[k] > 1 || hi[k] < 0 || hi[k] > 1)
-      return xg_fail(XG_EINVAL, who + ": halo widths must be 0 or 1");
-    if ((lo[k] || hi[k]) && (bc[k] < XG_BC_PERIODIC || bc[k] > XG_BC_EXTEND))
-      return xg_fail(XG_EINVAL, who + ": each padded axis needs a periodic / fill / extend boundary");
-    if (shape[d] == 0) return xg_fail(XG_EINVAL, who + ": empty operated axis");
-    app[d] = k;
-    out_shape[d] = shape[d] + lo[k] + hi[k] - 1;
+    app[axes[k]] = k;
+    out_shape[axes[k]] = shape[axes[k]] + lo[k] + hi[k] - 1;
   }
   // slab dim: the outermost non-operated dim of extent > 1, whose slabs hold every operated line whole; else the
   // outermost dim of extent > 1, an operated one (the dims in front of it have extent 1)
@@ -288,10 +272,28 @@ extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int n
   const size_t es = dtype == XG_F32 ? 4 : 8;
   const View3 vin = view3(ndim, shape, sd), vout = view3(ndim, out_shape, sd);
   ex.row_bytes = (vin.C * vin.R + vout.C * vout.R) * (int64_t)es;
+  // each stage's metric shapes: its input (pre) and output (post)
+  int64_t met_shape[2 * 3][XG_MAX_NDIM];
+  for (int m = 0; m < naxes; ++m)
+    for (int d = 0; d < ndim; ++d) {
+      met_shape[m][d] = app[d] >= 0 && app[d] < m ? out_shape[d] : shape[d];
+      met_shape[3 + m][d] = app[d] >= 0 && app[d] <= m ? out_shape[d] : shape[d];
+    }
   return spread(who.c_str(), device, vout.L, false, [&](int dev, int64_t r0, int64_t r1) -> int {
     Session ss;
-    int rc = ss.open(dev);
-    if (rc) return rc;
+    int rc2 = ss.open(dev);
+    if (rc2) return rc2;
+    const void* d_met[2 * 3] = {};  // pre[0..3), post[0..3) on this device
+    for (int m = 0; m < naxes && !rc2; ++m)
+      for (int w = 0; w < 2 && !rc2; ++w) {
+        const void* const* h = w ? post : pre;
+        const int64_t* st = (w ? post_strides : pre_strides) + m * ndim;
+        if (h && h[m])
+          rc2 = ss.upload((Aux)(kAuxStage0 + 3 * w + m), h[m], operand_span(st, met_shape[3 * w + m], ndim, es),
+                          &d_met[3 * w + m]);
+      }
+    if (!rc2 && (pre || post)) rc2 = ss.fence();
+    if (rc2) return rc2;
     const int64_t n = shape[sd];
     auto launch = [&](int64_t j0, int64_t j1, int64_t i0, int64_t i1, const SlabBufs& b, cudaStream_t st) -> int {
       int64_t sshape[XG_MAX_NDIM];
@@ -303,24 +305,57 @@ extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int n
         sbc[k] = bc[k];
       }
       const char* src = static_cast<const char*>(b.in);
+      int64_t s0 = j0;  // first input row of the slab along the cut dim
       if (ka >= 0) {
         // an inner slab edge reads its neighbour row, the field's own ends keep the call's boundary condition
         if (vin.C != 1) return xg_fail(XG_EINVAL, who + ": internal slab window error");
         Window w;
-        const int rc2 = read_window(who.c_str(), j0, j1, lo[ka], n, i0, i1, &w);
-        if (rc2) return rc2;
+        const int rc3 = read_window(who.c_str(), j0, j1, lo[ka], n, i0, i1, &w);
+        if (rc3) return rc3;
         slo[ka] = w.slo;
         shi[ka] = w.shi;
         if (!w.slo && !w.shi) sbc[ka] = XG_BC_NONE;
         src += (size_t)(w.s0 - i0) * vin.R * es;
         sshape[sd] = w.s1 - w.s0;
+        s0 = w.s0;
       } else {
         sshape[sd] = j1 - j0;
       }
-      return xg_stencil_multi(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc, fill_value, st);
+      if (!pre && !post)
+        return xg_stencil_multi(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc, fill_value, st);
+      // the slab's metrics: the cut dim at input rows (s0) before the stage that operates it, at result rows after
+      const void* met[2 * 3] = {};
+      for (int m = 0; m < naxes; ++m)
+        for (int w = 0; w < 2; ++w) {
+          const int i = 3 * w + m;
+          if (!d_met[i]) continue;
+          const int64_t row = (ka >= 0 && (w ? m < ka : m <= ka)) ? s0 : j0;
+          const int64_t stride = (w ? post_strides : pre_strides)[m * ndim + sd];
+          met[i] = static_cast<const char*>(d_met[i]) + (size_t)(row * stride) * es;
+        }
+      return xg_stencil_multi_weighted(dtype, src, b.out[0], ndim, sshape, naxes, axes, ops, slo, shi, sbc,
+                                       fill_value, met, pre_strides, met + 3, post_strides, st);
     };
     return ss.run(es, in, vin, 1, &out, &vout, launch, ex.rows(r0, r1));
   });
+}
+
+}  // namespace
+
+extern "C" int xg_stencil_multi_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape, int naxes,
+                                     const int* axes, const int* ops, const int* lo, const int* hi, const int* bc,
+                                     const double* fill_value, int device) {
+  return multi_host("xg_stencil_multi_host", dtype, in, out, ndim, shape, naxes, axes, ops, lo, hi, bc, fill_value,
+                    nullptr, nullptr, nullptr, nullptr, device);
+}
+
+extern "C" int xg_stencil_multi_weighted_host(int dtype, const void* in, void* out, int ndim, const int64_t* shape,
+                                              int naxes, const int* axes, const int* ops, const int* lo, const int* hi,
+                                              const int* bc, const double* fill_value, const void* const* pre,
+                                              const int64_t* pre_strides, const void* const* post,
+                                              const int64_t* post_strides, int device) {
+  return multi_host("xg_stencil_multi_weighted_host", dtype, in, out, ndim, shape, naxes, axes, ops, lo, hi, bc,
+                    fill_value, pre, pre_strides, post, post_strides, device);
 }
 
 // ---------------------------------------------------------------------------------------------------

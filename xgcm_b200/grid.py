@@ -565,16 +565,17 @@ class Grid:
         host_input = not unpacked.is_device
         array = unpacked.copy(deep=False)
         n_axes = len(axis)
+        weights = {ax: metric_weighted.get(ax) for ax in axis if metric_weighted.get(ax)}
         if (
             n_axes in (2, 3)
             and len(set(axis)) == n_axes
-            and not any(metric_weighted.get(ax) for ax in axis)
+            and (not weights or other_component is None)
             and _divide_by_metric_of is None
             and not isinstance(data, dict)
             and set(kwargs) <= {"padding", "fill_value"}
         ):
-            fused = self._fused_multi_axis(funcname, array, axis, to, kwargs)
-            if fused is None and other_component is None:  # a scalar field: no vector halo across a seam
+            fused = self._fused_multi_axis(funcname, array, axis, to, kwargs, weights)
+            if fused is None and other_component is None and not weights:  # a scalar field: no vector halo
                 fused = self._multi_axis_halo_host(funcname, array, axis, to, kwargs)
             if fused is not None:
                 return self._wrap_out(fused, as_xarray)
@@ -607,19 +608,26 @@ class Grid:
             array = array._replace(data=result_like(array.data, True))
         return self._wrap_out(array, as_xarray)
 
-    def _fused_multi_axis(self, funcname, array, axis, to, kwargs):
+    def _fused_multi_axis(self, funcname, array, axis, to, kwargs, weights=None):
         """All axes of a multi-axis diff / interp / min / max in ONE kernel launch
         (``xg_stencil_multi``): same values as the per-axis loop of grid.py:800-832, one read and
-        one write of the field instead of one pass per axis.  Returns None when the fused kernel
-        does not cover the case (then the caller runs the per-axis launches)."""
+        one write of the field instead of one pass per axis.  ``weights`` (axis name -> the
+        ``metric_weighted`` axes of its stage) gives each weighted stage the pre- and post-metric
+        the loop would take, ``get_metric`` of the stage's input and output dims
+        (``xg_stencil_multi_weighted``).  Returns None when the fused kernel does not cover the case
+        (then the caller runs the per-axis launches)."""
         from . import ops
         from .device import as_device_tensor, result_like
+        from .grid_ufunc import _ShapeProbe
 
         if self._face_connections is not None:
             return None  # halos come from other faces: per-axis pad + stencil
+        weights = weights or {}
         paddings = self._complete_user_kwargs_using_axis_defaults(kwargs.get("padding"), "padding")
         fills = self._complete_user_kwargs_using_axis_defaults(kwargs.get("fill_value"), "fill_value")
         specs, rename = [], {}
+        dims, shape = tuple(array.dims), list(array.shape)
+        stages = []  # per stage: its metric_weighted axes, input dims and shape, output dims and shape
         for ax_name in axis:
             t = _stencil_term(self, funcname, array, ax_name, to.get(ax_name), paddings, fills)
             if t.folded:
@@ -628,20 +636,42 @@ class Grid:
                 return None  # e.g. the opt-in extrapolate extension: per-axis path
             specs.append((t.axis_num, funcname, t.lo, t.hi, t.pad_mode if (t.lo or t.hi) else None, t.fill))
             rename[t.in_dim] = t.out_dim
+            out_dims = tuple(t.out_dim if d == t.in_dim else d for d in dims)
+            out_shape = list(shape)
+            out_shape[t.axis_num] += t.lo + t.hi - 1
+            stages.append((weights.get(ax_name), dims, shape, out_dims, out_shape))
+            dims, shape = out_dims, out_shape
         if array.shape[-1] < 32:
             return None  # tiny rows: the one-block-per-row kernel has nothing to chew on
+        stage_mets = [None if not w else (self.get_metric(_ShapeProbe(d, s), w), d,
+                                          self.get_metric(_ShapeProbe(od, os_), w), od)
+                      for w, d, s, od, os_ in stages]
+
+        def metrics(convert):
+            if not weights:
+                return {}
+            pre = [None if sm is None else convert(sm[0], sm[1]) for sm in stage_mets]
+            post = [None if sm is None else convert(sm[2], sm[3]) for sm in stage_mets]
+            return {"pre": pre, "post": post}
+
         out = None
         dev = self._device_for(array)
         if _is_host_float(array) and dev.type == "cuda":
             # numpy-backed field: slabs stream through the GPU (xg_stencil_multi_host), so input, result and the
             # device footprint need not fit in HBM together
+            x = np.asarray(array.data)
             try:
-                out = ops.stencil_multi_host(np.asarray(array.data), specs, device=self._host_device(array))
+                out = ops.stencil_multi_host(x, specs, device=self._host_device(array),
+                                             **metrics(lambda m, d: self._metric_host(m, d, x.dtype)))
             except NotImplementedError:
                 out = None  # a cut along an operated dim the slabs cannot pad: the whole field on the device
         if out is None:
             x, was_host = as_device_tensor(array.data, dev)
-            out = result_like(ops.stencil_multi(x, specs), was_host)
+            try:
+                y = ops.stencil_multi(x, specs, **metrics(lambda m, d: self._metric_tensor(m, d, x)))
+            except NotImplementedError:
+                return None  # a metric layout the weighted kernel does not address: per-axis launches
+            out = result_like(y, was_host)
         out_dims = tuple(rename.get(d, d) for d in array.dims)
         res = DataArray(out, dims=out_dims, name=array.name, attrs=array.attrs)
         return _reattach_coords([res], self, None, set(rename.values()), [array])[0]

@@ -171,10 +171,17 @@ def stencil2(
     return out
 
 
-def stencil_multi(x: torch.Tensor, specs: Sequence[Tuple[int, str, int, int, Optional[str], float]]) -> torch.Tensor:
+def stencil_multi(x: torch.Tensor, specs: Sequence[Tuple[int, str, int, int, Optional[str], float]], *,
+                  pre: Optional[Sequence[Optional[torch.Tensor]]] = None,
+                  post: Optional[Sequence[Optional[torch.Tensor]]] = None) -> torch.Tensor:
     """Fused chain of 2 or 3 single-axis stencils: ``specs`` = [(axis, op, lo, hi, padding, fill), ...]
     in application order.  Bit-identical to the corresponding sequence of :func:`stencil2` calls,
-    with one read and one write of the field (reference: one full pass per axis, grid.py:798-832)."""
+    with one read and one write of the field (reference: one full pass per axis, grid.py:798-832).
+
+    ``pre`` / ``post``: per stage, a metric that broadcasts against the stage's input / output (or None), as
+    :func:`stencil2` takes them (``metric_weighted``); the chain then runs ``xg_stencil_multi_weighted``, still one
+    launch.  NotImplementedError for a layout the weighted kernel does not address (two or more non-operated dims
+    after the last operated one)."""
     import ctypes as C
 
     lib = _capi.load()
@@ -185,23 +192,58 @@ def stencil_multi(x: torch.Tensor, specs: Sequence[Tuple[int, str, int, int, Opt
     shape = list(x.shape)
     axes, opc, los, his, bcs, fills = _stencil_specs(specs, x.dim(), fused=True)
     out_shape = _multi_out_shape(shape, axes, los, his)
+    pre, post = _stage_list(pre, len(specs), "pre"), _stage_list(post, len(specs), "post")
     if len(set(opc)) != 1:
         # mixed operators: not a Grid-level case; same result through the per-axis kernel
         out = x
-        for axis, op, lo, hi, padding, fill in specs:
-            out = stencil2(out, axis, op, lo, hi, padding if (lo or hi) else None, fill)
+        for k, (axis, op, lo, hi, padding, fill) in enumerate(specs):
+            out = stencil2(out, axis, op, lo, hi, padding if (lo or hi) else None, fill, pre=pre[k], post=post[k])
         return out
     out = torch.empty(out_shape, dtype=x.dtype, device=x.device)
     n = len(specs)
     IntArr, DblArr = C.c_int * n, C.c_double * n
+    weighted = any(m is not None for m in pre + post)
+    if weighted:
+        keep, met_args = [], []
+        for mets, shapes, what in ((pre, _stage_shapes(shape, axes, los, his, 0), "pre"),
+                                   (post, _stage_shapes(shape, axes, los, his, 1), "post")):
+            ptrs, strides = (C.c_void_p * n)(), []
+            for k, (m, s) in enumerate(zip(mets, shapes)):
+                mb, ptr, st = _operand(m, s, x, f"{what} metric of stage {k}")
+                keep.append(mb)
+                ptrs[k] = ptr
+                strides += list(st) if st is not None else [0] * len(shape)
+            met_args += [ptrs, _capi.i64_array(strides)]
     if out.numel():
+        args = (_dtype_code(x), x.data_ptr(), out.data_ptr(), x.dim(), _capi.i64_array(shape), n,
+                IntArr(*axes), IntArr(*opc), IntArr(*los), IntArr(*his), IntArr(*bcs), DblArr(*fills))
         with torch.cuda.device(x.device):
-            rc = lib.xg_stencil_multi(
-                _dtype_code(x), x.data_ptr(), out.data_ptr(), x.dim(), _capi.i64_array(shape), n,
-                IntArr(*axes), IntArr(*opc), IntArr(*los), IntArr(*his), IntArr(*bcs), DblArr(*fills),
-                _stream_ptr(x),
-            )
+            if weighted:
+                rc = lib.xg_stencil_multi_weighted(*args, *met_args, _stream_ptr(x))
+            else:
+                rc = lib.xg_stencil_multi(*args, _stream_ptr(x))
         _capi.check(rc)
+    return out
+
+
+def _stage_list(mets, n, what):
+    """``pre`` / ``post`` of a fused chain as a list of one entry (a metric or None) per stage."""
+    if mets is None:
+        return [None] * n
+    mets = list(mets)
+    if len(mets) != n:
+        raise ValueError(f"{what}: one metric (or None) per stage, got {len(mets)} for {n} stages")
+    return mets
+
+
+def _stage_shapes(shape, axes, los, his, after):
+    """Shape of each stage's input (after=0) or output (after=1) of a fused chain."""
+    out, cur = [], list(shape)
+    for axis, lo, hi in zip(axes, los, his):
+        nxt = list(cur)
+        nxt[axis] = cur[axis] + lo + hi - 1
+        out.append(nxt if after else cur)
+        cur = nxt
     return out
 
 
@@ -940,11 +982,15 @@ def stencil2_host_multi(x: np.ndarray, specs, outs=None, device: HostDevice = No
 
 
 def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, Optional[str], float]],
-                       device: HostDevice = None) -> np.ndarray:
+                       device: HostDevice = None, *, pre: Optional[Sequence[Optional[np.ndarray]]] = None,
+                       post: Optional[Sequence[Optional[np.ndarray]]] = None) -> np.ndarray:
     """Host twin of :func:`stencil_multi` (``xg_stencil_multi_host``): slabs of the outermost non-operated dim of
     extent > 1 stream through the GPU, one fused launch each.  Raises NotImplementedError for what the slabs do not
     cover (mixed operators; an outer / inner shift or a periodic boundary along the cut dim when every dim of extent
-    > 1 is operated) — callers then use :func:`stencil_multi`."""
+    > 1 is operated) — callers then use :func:`stencil_multi`.
+
+    ``pre`` / ``post``: per-stage host metrics as :func:`stencil_multi` takes them (``xg_stencil_multi_weighted_host``:
+    uploaded whole once per device, each slab's launch offset into them)."""
     import ctypes as C
 
     lib = _capi.load()
@@ -956,11 +1002,27 @@ def stencil_multi_host(x: np.ndarray, specs: Sequence[Tuple[int, str, int, int, 
     out = pinned_empty(_multi_out_shape(shape, axes, los, his), x.dtype)
     n = len(specs)
     IntArr, DblArr = C.c_int * n, C.c_double * n
+    pre, post = _stage_list(pre, n, "pre"), _stage_list(post, n, "post")
+    weighted = any(m is not None for m in pre + post)
+    keep, met_args = [], []
+    if weighted:
+        for mets, shapes, what in ((pre, _stage_shapes(shape, axes, los, his, 0), "pre"),
+                                   (post, _stage_shapes(shape, axes, los, his, 1), "post")):
+            ptrs, strides = (C.c_void_p * n)(), []
+            for k, (m, s) in enumerate(zip(mets, shapes)):
+                mh, ptr, st = _host_operand(m, s, x.dtype, f"{what} metric of stage {k}")
+                keep.append(mh)
+                ptrs[k] = ptr
+                strides += list(st) if st is not None else [0] * len(shape)
+            met_args += [ptrs, _capi.i64_array(strides)]
     dev = host_device_arg(device)
     if out.size:
-        rc = lib.xg_stencil_multi_host(
-            _capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), n,
-            IntArr(*axes), IntArr(*opc), IntArr(*los), IntArr(*his), IntArr(*bcs), DblArr(*fills), dev)
+        args = (_capi.dtype_code(x.dtype), x.ctypes.data, out.ctypes.data, x.ndim, _capi.i64_array(shape), n,
+                IntArr(*axes), IntArr(*opc), IntArr(*los), IntArr(*his), IntArr(*bcs), DblArr(*fills))
+        if weighted:
+            rc = lib.xg_stencil_multi_weighted_host(*args, *met_args, dev)
+        else:
+            rc = lib.xg_stencil_multi_host(*args, dev)
         _capi.check(rc)
     return out
 
